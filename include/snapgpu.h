@@ -88,7 +88,7 @@ typedef struct snapgpu_params {
     int32_t  noTruncation;
     int32_t  noEditDistance;            /* -ne */
     int32_t  noBandedAffineGap;
-    int32_t  altAwareness;              /* -ea- turns off (1) */
+    int32_t  altAwareness;              /* -A- turns off (1) */
     int32_t  maxScoreGapToPreferNonAltAlignment; /* (64) */
     int32_t  explorePopularSeeds;       /* -x (0) */
     int32_t  stopOnFirstHit;            /* -f (0) */
@@ -319,7 +319,7 @@ int  snapgpu_align_single_secondary_device(snapgpu_aligner *a, int64_t n, const 
 /*
  * Paired-end aligner handle: the ChimericPairedEndAligner(IntersectingPairedEndAligner) stack that
  * PairedAlignerContext::runIterationThread builds per thread (reference SNAPLib/PairedAligner.cpp:547-638).
- * Scope: no secondary results (-om unset); an index with ALT contigs only with params->altAwareness = 0 (-ea-): ALT-aware pairing is not implemented.  Soft clipping (the default) runs the Hamming / gapless
+ * Scope: no secondary results (-om unset); on an index with ALT contigs the pairing is ALT-aware (two score sets, liftover of ALT pairs onto their primary contig) unless params->altAwareness = 0 (-A-).  Soft clipping (the default) runs the Hamming / gapless
  * passes of both aligners (IntersectingPairedEndAligner::alignHamming, BaseAligner::AlignRead(useHamming) +
  * alignAffineGap); useSoftClipping = 0 is `snap paired -hc`.
  */

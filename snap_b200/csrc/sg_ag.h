@@ -13,6 +13,8 @@ struct SgAgParams {
     int matchReward, subPenalty /* negative */, gapOpenPenalty /* open+extend */, gapExtendPenalty, fivePrimeEndBonus, threePrimeEndBonus;
     int usePacked;                   // device: take the specialised forms (packed s16x2 for unbanded problems, sg_warp_ag_rows_banded4 for
                                      // narrow bands); results are identical either way, which is faster depends on the kernel (DESIGN.md 6)
+    int altLiftover;                 // the reference's useAltLiftover: no quality-aware end adjustment (AffineGapVectorized.h:691, 1212).
+                                     // Only the general form honours it; its callers set usePacked = 0.
 };
 
 SG_HD SgAgParams sg_ag_params(int matchReward, int subPenalty, int gapOpen, int gapExtend, int five, int three)
@@ -20,7 +22,7 @@ SG_HD SgAgParams sg_ag_params(int matchReward, int subPenalty, int gapOpen, int 
     SgAgParams p;                    // AffineGapVectorized::init, :105-133
     p.matchReward = matchReward; p.subPenalty = -subPenalty; p.gapOpenPenalty = gapOpen + gapExtend;
     p.gapExtendPenalty = gapExtend; p.fivePrimeEndBonus = five; p.threePrimeEndBonus = three;
-    p.usePacked = 0;
+    p.usePacked = 0; p.altLiftover = 0;
     return p;
 }
 
@@ -146,7 +148,7 @@ SG_HDN void sg_ag_finish(const SgTables &T, const SgAgParams &P, const SgAgLayou
                     oPat = patternOffsetAdj - 1; oText = textOffsetAdj - 1;
                 }
             }
-            if (oPat == bestLocalAlignmentPatternOffset && oText == bestLocalAlignmentTextOffset) {
+            if (oPat == bestLocalAlignmentPatternOffset && oText == bestLocalAlignmentTextOffset && !P.altLiftover) {
                 patternOffsetAdj = oPat;
                 while (patternOffsetAdj != patternLen - 1 && (int8_t)quality[patternOffsetAdj] >= 65 && (int8_t)quality[patternOffsetAdj + 1] >= 65) {
                     patternOffsetAdj += 1;

@@ -62,6 +62,12 @@ struct SgIndexView {
     uint32_t pad0;
     const uint64_t *buckets;         // [nBuckets * 4]
     uint64_t nBuckets;
+    // ALT liftover (Genome::Contig::projBeginningLocation / isProjRC / projCigarOps, Genome.cpp:348-403), NULL for an index
+    // without ALT contigs: projStart[c] as the Genome file gives it; projRC[c]; projOps[0, nContigs] = where contig c's ops
+    // begin in projOps (absolute index; c's ops end where c+1's begin), followed by the ops, each count << 8 | action character
+    const int64_t  *projStart;
+    const uint8_t  *projRC;
+    const uint32_t *projOps;
 };
 #define SG_LAYOUT_SNAP 0
 #define SG_LAYOUT_BUCKET 1

@@ -6,6 +6,7 @@
 #include <string.h>
 #include <math.h>
 #include <limits.h>
+#include <algorithm>
 #include <string>
 #include <vector>
 #include "sg_common.h"
@@ -20,6 +21,10 @@ struct SgHostIndex {
     std::vector<uint8_t>  contigIsAlt;
     std::vector<int32_t>  contigOriginal;   // Genome::Contig::originalContigNumber (order in the FASTA; what sorted output is ordered by)
     std::vector<std::string> contigName;
+    // ALT liftover data of each contig line (SgIndexView::projStart / projRC / projOps); empty when no contig is ALT
+    std::vector<int64_t>  projStart;
+    std::vector<uint8_t>  projRC;
+    std::vector<uint32_t> projOps;
     int64_t  nBases = 0, altFirstLocation = LLONG_MAX;
     uint32_t seedLen = 0, keyBytes = 0, nTables = 0, large = 0, entryBytes = 0, chromosomePadding = 0, locationSize = 4;
     uint32_t invalidValue = 0xffffffffu;
@@ -37,6 +42,9 @@ struct SgHostIndex {
         v.nContigs = (uint32_t)contigStart.size(); v.seedLen = seedLen; v.keyBytes = keyBytes; v.nTables = nTables;
         v.large = large; v.entryBytes = entryBytes; v.chromosomePadding = chromosomePadding; v.invalidValue = invalidValue;
         v.layout = layout; v.pad0 = 0; v.buckets = buckets.empty() ? (const uint64_t *)0 : buckets.data(); v.nBuckets = nBuckets;
+        v.projStart = projStart.empty() ? (const int64_t *)0 : projStart.data();
+        v.projRC = projRC.empty() ? (const uint8_t *)0 : projRC.data();
+        v.projOps = projOps.empty() ? (const uint32_t *)0 : projOps.data();
         return v;
     }
 };
@@ -86,6 +94,8 @@ static inline bool sg_load_index_directory(const std::string &dir, SgHostIndex &
         p = nl + 1;
         ix.nBases = nBases;
         ix.contigStart.clear(); ix.contigIsAlt.clear(); ix.contigName.clear(); ix.contigOriginal.clear();
+        ix.projStart.clear(); ix.projRC.clear();
+        std::vector<uint32_t> projOpBegin, ops;
         for (int i = 0; i < nContigs; i++) {
             nl = (const char *)memchr(p, '\n', endp - p);
             if (!nl) { err = "Genome contig line truncated"; return false; }
@@ -101,7 +111,32 @@ static inline bool sg_load_index_directory(const std::string &dir, SgHostIndex &
             ix.contigOriginal.push_back(origNum);
             if (nameLen < 0 || (long long)nameLen > (long long)(nl - q)) { err = "Genome contig line: name length runs past the line"; return false; }
             ix.contigName.push_back(std::string(q, (size_t)nameLen));
+            // the projection CIGAR follows the name; a length of 1 is the "*" of a contig without a liftover line (Genome.cpp:380-401)
+            ix.projStart.push_back(projStart);
+            ix.projRC.push_back(0);
+            projOpBegin.push_back((uint32_t)ops.size());
+            if (cigarLen > 1) {
+                const char *c = q + nameLen + 1;
+                if (c + cigarLen > nl) { err = "Genome contig line: projection CIGAR runs past the line"; return false; }
+                const char *ce = c + cigarLen;
+                while (c < ce) {
+                    long long count = 0; const char *d = c;
+                    while (c < ce && *c >= '0' && *c <= '9') { count = count * 10 + (*c - '0'); c++; if (count > 0x7fffffLL) break; }
+                    if (c == d || c >= ce || count > 0x7fffffLL || !strchr("MIDNSHP=X", *c)) { err = "Genome contig line: malformed projection CIGAR"; return false; }
+                    ops.push_back(((uint32_t)count << 8) | (uint8_t)*c);
+                    c++;
+                }
+                ix.projRC.back() = (projRC & 1) ? 1 : 0;       // GENOME_FLAG_ALT_PROJ_CONTIG_IS_RC
+            }
             p = nl + 1;
+        }
+        projOpBegin.push_back((uint32_t)ops.size());
+        ix.projOps.clear();
+        if (std::find(ix.contigIsAlt.begin(), ix.contigIsAlt.end(), (uint8_t)1) == ix.contigIsAlt.end()) {
+            ix.projStart.clear(); ix.projRC.clear();        // nothing can be lifted over
+        } else {
+            for (size_t c = 0; c < projOpBegin.size(); c++) ix.projOps.push_back((uint32_t)projOpBegin.size() + projOpBegin[c]);
+            ix.projOps.insert(ix.projOps.end(), ops.begin(), ops.end());
         }
         if ((long long)(endp - p) != nBases) { err = "Genome: base count does not match file size"; return false; }
         ix.basesPadded.assign((size_t)nBases + 2 * SG_N_PADDING, (uint8_t)'n');

@@ -8,14 +8,72 @@
 // cross-checks with the single-end aligner of sg_align.h.
 // alignHamming (:1441-2487) is the same three phases with gapless (Hamming + end clipping) scoring
 // (scoreLocationWithHammingDistance :3401-3497); it is restated here as the `hamming` mode of the same function.
-// Configuration covered: no secondary results (-om unset), no ALT contigs.
+// Configuration covered: no secondary results (-om unset).  ALT awareness is covered in full: the two score sets, firstALTResult
+// (the best pair when it lies on ALT contigs and a non-ALT one is emitted; kept per pair, not written out: -ea is not supported) and
+// the liftover of ALT pairs onto their primary contig (alignAffineGap :2865-2966).
 #pragma once
+#include <limits.h>
 #include "sg_align.h"
+#include "sg_cigar.h"
 
 #define SG_MAX_MAX_SEEDS 30          // IntersectingPairedEndAligner.h:216
 #define SG_PAIRED_MERGE_DIST 31      // maxMergeDistance, IntersectingPairedEndAligner.cpp:3990
 #define SG_LOCATION_NOT_YET_SCORED (-2)
 #define SG_MAX_AG_CANDIDATES 4096    // PairedAligner.cpp:570-573
+// bit of sg_paired_align_stage1's return value: the last of the nLVCand phase-4 candidates it hands over is the pair's firstALTResult
+#define SG_STAGE_ALT_RESULT 4
+
+// Genome::getProjContigNumAtLocation, getContigProjSpan, getProjLocation, isProjContigRC (Genome.cpp:634-715) over SgIndexView::projStart /
+// projRC / projOps.  Only called on an index with ALT contigs (projStart != NULL).
+SG_HD int sg_proj_contig_num_at(const SgIndexView &ix, int64_t location)
+{
+    const int p = sg_contig_at(ix, ix.projStart[sg_contig_at(ix, location)]);
+    return p < 0 ? -2 : p;           // no contig there (a contig without a liftover line): the reference's number then matches no contig either
+}
+
+SG_HD int64_t sg_contig_proj_span(const SgIndexView &ix, int contig)
+{
+    int64_t offset = 0;
+    const uint32_t b = ix.projOps[contig], e = ix.projOps[contig + 1];
+    for (uint32_t i = b; i < e; i++) {
+        const char action = (char)(ix.projOps[i] & 0xff);
+        const int64_t count = (int64_t)(ix.projOps[i] >> 8);
+        if (i == b ? (action != 'S' && action != 'H') : (action == 'M' || action == 'I')) offset += count;
+    }
+    return offset;
+}
+
+// the bwa-postalt walk; `invalid` (InvalidGenomeLocation) inside a soft / hard clip of the ALT contig
+SG_HD int64_t sg_proj_location(const SgIndexView &ix, int64_t location, int alnSpan, int64_t invalid)
+{
+    const int contig = sg_contig_at(ix, location);
+    const int64_t begin = ix.contigStart[contig];
+    const int64_t offset = !ix.projRC[contig] ? location - begin : sg_contig_proj_span(ix, contig) - (location - begin + alnSpan);
+    int64_t projOffset = 0, x = 0, y = 0;        // x: primary (REF), y: ALT
+    uint32_t i = ix.projOps[contig];
+    const uint32_t e = ix.projOps[contig + 1];
+    if (i < e && ((ix.projOps[i] & 0xff) == 'S' || (ix.projOps[i] & 0xff) == 'H')) i++;
+    for (; i < e; i++) {
+        const char action = (char)(ix.projOps[i] & 0xff);
+        const int64_t count = (int64_t)(ix.projOps[i] >> 8);
+        if (action == 'M') {
+            if (y <= offset && offset < y + count) { projOffset = x + (offset - y); break; }
+            x += count; y += count;
+        } else if (action == 'D') {
+            x += count;
+        } else if (action == 'I') {
+            if (y <= offset && offset < y + count) { projOffset = x; break; }
+            y += count;
+        } else if (action == 'S' || action == 'H') {
+            if (y <= offset && offset < y + count) { projOffset = -1; break; }
+            y += count;
+        }
+    }
+    if (projOffset == -1) return invalid;
+    return ix.projStart[contig] + projOffset;
+}
+
+SG_HD int sg_proj_contig_rc(const SgIndexView &ix, int64_t location) { return ix.projRC[sg_contig_at(ix, location)] ? SNAPGPU_RC : SNAPGPU_FORWARD; }
 
 struct SgPairedParams {
     int32_t  minSpacing; uint32_t maxSpacing; uint32_t maxBigHits; uint32_t poolSize; uint32_t maxSeedsSingleEnd; uint32_t maxKForIndels;
@@ -283,7 +341,7 @@ struct SgPairedScratch {
     SgMateCandidate *mates[2];       // [poolSize/2] each
     SgMergeAnchor *anchors;          // [poolSize]
     int32_t *scoreLists;             // [MAX_K + extraSearchDepth + 2] heads (pool index or -1)
-    snapgpu_paired_result *lvCandidates;   // [agCandCap]
+    snapgpu_paired_result *lvCandidates;   // [agCandCap + 1]: the phase-4 candidates, then the pair's firstALTResult (SgPairedAligner::altResult)
     snapgpu_single_result *singleCandidates;   // [agCandCap] candidatesForAffineGap of the single-end Hamming pass
     uint8_t *agBt[2];                // the Chimeric aligner's own AffineGapVectorized objects used by the intersecting aligner
 };
@@ -298,7 +356,7 @@ SG_HD size_t sg_paired_scratch_bytes(const SgParams &p, const SgPairedParams &pp
     b += 2 * sg_align_up(sizeof(SgMateCandidate) * (size_t)(pp.poolCap / 2), 256);
     b += sg_align_up(sizeof(SgMergeAnchor) * (size_t)pp.poolCap, 256);
     b += sg_align_up(4 * (SG_MAX_K + 64), 256);
-    b += sg_align_up(sizeof(snapgpu_paired_result) * (size_t)pp.agCandCap, 256);
+    b += sg_align_up(sizeof(snapgpu_paired_result) * ((size_t)pp.agCandCap + 1), 256);
     b += sg_align_up(sizeof(snapgpu_single_result) * (size_t)pp.agCandCap, 256);
     b += 2 * sg_align_up(agRows * agCols, 256);
     return b;
@@ -322,7 +380,7 @@ SG_HD void sg_paired_scratch_carve(const SgParams &p, const SgPairedParams &pp, 
     for (int k = 0; k < 2; k++) { s->mates[k] = (SgMateCandidate *)q; q += sg_align_up(sizeof(SgMateCandidate) * (size_t)(pp.poolCap / 2), 256); }
     s->anchors = (SgMergeAnchor *)q; q += sg_align_up(sizeof(SgMergeAnchor) * (size_t)pp.poolCap, 256);
     s->scoreLists = (int32_t *)q; q += sg_align_up(4 * (SG_MAX_K + 64), 256);
-    s->lvCandidates = (snapgpu_paired_result *)q; q += sg_align_up(sizeof(snapgpu_paired_result) * (size_t)pp.agCandCap, 256);
+    s->lvCandidates = (snapgpu_paired_result *)q; q += sg_align_up(sizeof(snapgpu_paired_result) * ((size_t)pp.agCandCap + 1), 256);
     s->singleCandidates = (snapgpu_single_result *)q; q += sg_align_up(sizeof(snapgpu_single_result) * (size_t)pp.agCandCap, 256);
     s->agBt[0] = q; q += sg_align_up(agRows * agCols, 256);
     s->agBt[1] = q; q += sg_align_up(agRows * agCols, 256);
@@ -351,6 +409,9 @@ struct SgPairedAligner {
     snapgpu_paired_result wsKey;
 
     SG_HD bool isALT(int64_t loc) const { return loc >= ix->altFirstLocation; }
+    // the pair's firstALTResult.  Read only where its status is not NotFound -- but for popularSeedsSkipped, which the phase-4 emission takes
+    // from it as it stands (:2842), so that one is reset per pair too
+    SG_HD snapgpu_paired_result *altResult() const { return ps.lvCandidates + pp->agCandCap; }
     SG_HD bool isSeedUsed(int64_t i) const { return (ps.seedUsed[i / 8] & (1 << (i % 8))) != 0; }
     SG_HD void setSeedUsed(int64_t i) { ps.seedUsed[i / 8] |= (uint8_t)(1 << (i % 8)); }
     SG_HD static int setPairDirection(uint32_t whichSetPair, uint32_t whichRead) { return whichSetPair == 0 ? (int)whichRead : 1 - (int)whichRead; }
@@ -581,7 +642,10 @@ SG_HDN bool sg_paired_align_lv(SgPairedAligner &P, const uint8_t *const readBase
     const int maxK = P.maxK;
     const int esd = (int)pr.extraSearchDepth;
     const int maxLVCand = pr.useAffineGap ? (int)pp.agCandCap : 0;
+    snapgpu_paired_result *alt = P.altResult();
 
+    alt->status[0] = alt->status[1] = SNAPGPU_NOT_FOUND;
+    if (!hamming) alt->refSpan[0] = alt->refSpan[1] = 0;
     result->clippingForReadAdjustment[0] = result->clippingForReadAdjustment[1] = 0;
     result->usedAffineGapScoring[0] = result->usedAffineGapScoring[1] = 0;
     result->basesClippedBefore[0] = result->basesClippedBefore[1] = 0;
@@ -958,32 +1022,140 @@ SG_HDN bool sg_paired_align_lv(SgPairedAligner &P, const uint8_t *const readBase
             result->status[w] = SNAPGPU_NOT_FOUND; result->clippingForReadAdjustment[w] = 0; result->usedAffineGapScoring[w] = 0; result->usedGaplessClipping[w] = 0;
             result->basesClippedBefore[w] = 0; result->basesClippedAfter[w] = 0; result->agScore[w] = SG_SCORE_ABOVE_LIMIT; result->seedOffset[w] = 0;
             result->lvIndels[w] = 0; result->popularSeedsSkipped[w] = popularSeedsSkipped[w]; result->matchProbability[w] = 0.0;
+            alt->status[w] = SNAPGPU_NOT_FOUND;
         }
         result->probabilityAllPairs = 0.0;
     } else {
         emit->fillInResult(T, result, popularSeedsSkipped);
+        if (pr.altAwareness && emit == &nonAlt &&
+            (all.bestResultGenomeLocation[0] != nonAlt.bestResultGenomeLocation[0] || all.bestResultGenomeLocation[1] != nonAlt.bestResultGenomeLocation[1])) {
+            all.fillInResult(T, alt, popularSeedsSkipped);
+            alt->supplementary[0] = alt->supplementary[1] = 1;
+        } else {
+            alt->status[0] = alt->status[1] = SNAPGPU_NOT_FOUND;
+        }
     }
     for (int w = 0; w < 2; w++) result->scorePriorToClipping[w] = result->score[w];
     return true;
 }
 
-// IntersectingPairedEndAligner::alignAffineGap (:2489-2969), phase 4.  No ALT contigs => firstALTResult is always NotFound.
+// IntersectingPairedEndAligner::scoreLocationWithAffineGapLiftover (:2970-3118): the whole read from the projected start, forward and then back
+// over what the forward pass aligned, with useAltLiftover set.  Liftover is rare, so it takes the general affine-gap form (usePacked = 0), the
+// only one that honours the flag.  The reference counts no affine-gap call here.
+template <int AGM = 0>
+SG_HDN void sg_paired_score_location_ag_liftover(SgPairedAligner &P, uint32_t whichRead, int direction, int64_t genomeLocation, int scoreLimit, int *score,
+                                                 double *matchProbability, int *genomeLocationOffset, int *basesClippedBefore, int *basesClippedAfter,
+                                                 int *agScore, int *genomeSpan)
+{
+    const SgIndexView &ix = *P.ix; const SgParams &pr = *P.pr; const SgTables &T = *P.tb;
+    const int readLen = (int)P.readLen[whichRead];
+    const int64_t genomeDataLength = (int64_t)readLen + SG_MAX_K;
+    const uint8_t *data = sg_get_substring(ix, genomeLocation, genomeDataLength);
+    *genomeLocationOffset = 0;
+    *genomeSpan = 0;
+    if (data == (const uint8_t *)0) { *score = SG_SCORE_ABOVE_LIMIT; *matchProbability = 0; *genomeLocationOffset = 0; *agScore = SG_SCORE_ABOVE_LIMIT; return; }
+    *basesClippedBefore = 0; *basesClippedAfter = 0;
+    SgScratch sc = P.single->sc;
+    sc.agBt[0] = P.ps.agBt[0]; sc.agBt[1] = P.ps.agBt[1];
+    SgAgParams ag = P.ag;
+    ag.usePacked = 0; ag.altLiftover = 1;
+    SgAgResult ar;
+    int patternLen = readLen;
+    bool banded = (patternLen >= (3 * (2 * scoreLimit + 1))) && !pr.noBandedAffineGap;
+    ar.textOffset = 0; ar.patternOffset = 0; ar.nEdits = 0; ar.matchProbability = 1.0; ar.agScore = -1;
+    sg_ag_dispatch<AGM>(T, sc, ag, 1, banded, data, (int)genomeDataLength, P.readData[whichRead][direction], P.readQual[whichRead][direction], patternLen, scoreLimit,
+                        readLen, direction != 0, P.pp->useSoftClip != 0, &ar, sg_lane());
+    const int textRem = ar.textOffset, score1 = ar.nEdits;
+    *basesClippedAfter = ar.patternOffset;
+    if (score1 != SG_SCORE_ABOVE_LIMIT && score1 <= SG_MAX_K - 1) {
+        const int limitLeft = score1;
+        patternLen = readLen - *basesClippedAfter;
+        banded = (patternLen >= (3 * (2 * limitLeft + 1))) && !pr.noBandedAffineGap;
+        ar.textOffset = 0; ar.patternOffset = 0; ar.nEdits = 0; ar.matchProbability = 1.0; ar.agScore = -1;
+        sg_ag_dispatch<AGM>(T, sc, ag, -1, banded, data + readLen - textRem, readLen - textRem, P.ps.revRead[whichRead][direction] + *basesClippedAfter,
+                            P.readQual[whichRead][1 - direction] + *basesClippedAfter, patternLen, limitLeft, readLen, direction != 0, P.pp->useSoftClip != 0, &ar, sg_lane());
+        *basesClippedBefore = ar.patternOffset;
+        if (ar.nEdits == SG_SCORE_ABOVE_LIMIT || ar.nEdits > SG_MAX_K - 1) {
+            *score = SG_SCORE_ABOVE_LIMIT; *genomeLocationOffset = 0; *agScore = -1;
+        } else {
+            *score = ar.nEdits;
+            *agScore = ar.agScore - readLen;
+            *matchProbability = ar.matchProbability;
+            *genomeLocationOffset = *basesClippedAfter + ar.textOffset - textRem;
+            *genomeSpan = readLen - textRem - *genomeLocationOffset;
+        }
+    } else {
+        *score = SG_SCORE_ABOVE_LIMIT; *genomeLocationOffset = 0; *agScore = -1;
+    }
+}
+
+// The end of alignAffineGap (:2865-2966), soft clipping on: a pair on ALT contigs, or an ALT pair (firstALTResult) that beats the emitted one and
+// projects to another contig, is projected onto the primary contig and rescored there; if either end fails, the result stays as it was.
+template <int AGM = 0>
+SG_HDN void sg_paired_alt_liftover(SgPairedAligner &P, snapgpu_paired_result *result)
+{
+    const SgIndexView &ix = *P.ix;
+    const snapgpu_paired_result *alt = P.altResult();
+    int bestAltScore = INT_MAX, bestResScore = INT_MAX, altProjContigNum = -1, resContigNum = -1;
+    bool isResultALT = false;
+    if (alt->status[0] != SNAPGPU_NOT_FOUND && alt->status[1] != SNAPGPU_NOT_FOUND) {
+        bestAltScore = alt->score[0] + alt->score[1];
+        altProjContigNum = sg_proj_contig_num_at(ix, alt->location[0]);
+    }
+    if (result->status[0] != SNAPGPU_NOT_FOUND && result->status[1] != SNAPGPU_NOT_FOUND) {
+        bestResScore = result->score[0] + result->score[1];
+        resContigNum = sg_contig_at(ix, result->location[0]);
+        isResultALT = P.isALT(result->location[0]) && P.isALT(result->location[1]);
+    }
+    if (!(((bestAltScore < bestResScore) && (altProjContigNum != resContigNum)) || isResultALT)) return;
+    const snapgpu_paired_result *src = isResultALT ? result : alt;
+    const int projDirection = sg_proj_contig_rc(ix, src->location[0]);     // orientation of the ALT contig against its primary one
+    int newDirection[2], newSeedOffset[2], newMapq[2];
+    int64_t newStart[2];
+    for (int r = 0; r < 2; r++) {
+        newDirection[r] = (src->direction[r] != projDirection) ? SNAPGPU_RC : SNAPGPU_FORWARD;
+        newSeedOffset[r] = (newDirection[r] != src->direction[r]) ? (int)P.readLen[r] - src->seedOffset[r] - 1 : src->seedOffset[r];
+        newStart[r] = sg_proj_location(ix, src->location[r], src->refSpan[r], P.invalidLocation);
+        newMapq[r] = isResultALT ? (src->mapq[r] <= 3 ? 70 : src->mapq[r]) : src->mapq[r];
+    }
+    if (newStart[0] == P.invalidLocation || newStart[1] == P.invalidLocation) return;
+    snapgpu_paired_result &resultBeforeLiftover = P.wsKey;           // (the phase-4 sort is over)
+    resultBeforeLiftover = *result;
+    for (int r = 0; r < 2; r++) {
+        int genomeOffset;
+        result->usedAffineGapScoring[r] = 1;
+        result->liftover[r] = 1;
+        result->direction[r] = newDirection[r];
+        result->location[r] = newStart[r];
+        result->seedOffset[r] = newSeedOffset[r];
+        result->mapq[r] = newMapq[r];
+        sg_paired_score_location_ag_liftover<AGM>(P, (uint32_t)r, result->direction[r], result->location[r], SG_MAX_K - 1, &result->score[r], &result->matchProbability[r],
+                                                  &genomeOffset, &result->basesClippedBefore[r], &result->basesClippedAfter[r], &result->agScore[r], &result->refSpan[r]);
+        if (result->score[r] != SG_SCORE_ABOVE_LIMIT && result->score[r] <= SG_MAX_K - 1) result->location[r] += genomeOffset;
+        else result->status[r] = SNAPGPU_NOT_FOUND;
+    }
+    if (result->status[0] == SNAPGPU_NOT_FOUND || result->status[1] == SNAPGPU_NOT_FOUND) *result = resultBeforeLiftover;
+}
+
+// IntersectingPairedEndAligner::alignAffineGap (:2489-2969), phase 4, with the pair's firstALTResult (P.altResult()).
 template <int AGM = 0>
 SG_HDN void sg_paired_align_ag(SgPairedAligner &P, snapgpu_paired_result *result, int *nLVCandidatesForAffineGap)
 {
     const SgParams &pr = *P.pr; const SgPairedParams &pp = *P.pp; const SgTables &T = *P.tb;
     SgPairedScratch &ps = P.ps;
+    snapgpu_paired_result *alt = P.altResult();
     if (result->status[0] == SNAPGPU_NOT_FOUND || result->status[1] == SNAPGPU_NOT_FOUND) return;
     if (P.readLen[0] < P.ix->seedLen || P.readLen[1] < P.ix->seedLen) return;
     // the RC / reversed strings built by alignLandauVishkin are still valid (same reads); the N check passed there
     const int maxK = P.maxK, esd = (int)pr.extraSearchDepth;
     const int maxKForSameAlignment = pr.gapOpenPenalty / (pr.subPenalty - pr.gapExtendPenalty);
     const int bestPairScore = result->score[0] + result->score[1];
-    int scoreLimit;
-    if (result->usedGaplessClipping[0] || result->usedGaplessClipping[1]) scoreLimit = SG_MAX_K - 1; else scoreLimit = maxK + esd;
+    int scoreLimit, scoreLimitALT;
+    if (result->usedGaplessClipping[0] || result->usedGaplessClipping[1]) scoreLimit = scoreLimitALT = SG_MAX_K - 1; else scoreLimit = scoreLimitALT = maxK + esd;
     int genomeOffset[2] = {0, 0};
     bool skipAffineGap[2] = {false, false};
     const double oldPairProbabilityBestResult = result->matchProbability[0] * result->matchProbability[1];
+    const double oldPairProbabilityBestResultALT = (alt->status[0] != SNAPGPU_NOT_FOUND) ? alt->matchProbability[0] * alt->matchProbability[1] : 0.0;
 
     for (int r = 0; r < 2; r++) {
         if (result->usedGaplessClipping[r] || result->score[r] > maxKForSameAlignment) {
@@ -998,6 +1170,20 @@ SG_HDN void sg_paired_align_ag(SgPairedAligner &P, snapgpu_paired_result *result
             } else {
                 result->status[r] = SNAPGPU_NOT_FOUND;
             }
+            // the ALT pair's end is rescored only where the result's is, under its own limit (:2618-2644)
+            if (alt->status[r] != SNAPGPU_NOT_FOUND && (alt->usedGaplessClipping[r] || alt->score[r] > maxKForSameAlignment)) {
+                alt->usedAffineGapScoring[r] = 1;
+                if (!alt->usedGaplessClipping[r]) scoreLimitALT = scoreLimitALT > alt->score[r] ? scoreLimitALT : alt->score[r];
+                sg_paired_score_location_ag<AGM>(P, (uint32_t)r, alt->direction[r], alt->origLocation[r], (uint32_t)alt->seedOffset[r], scoreLimitALT, &alt->score[r],
+                                                 &alt->matchProbability[r], &genomeOffset[r], &alt->basesClippedBefore[r], &alt->basesClippedAfter[r],
+                                                 &alt->agScore[r], &alt->refSpan[r]);
+                if (alt->score[r] != SG_SCORE_ABOVE_LIMIT) {
+                    alt->location[r] = alt->origLocation[r] + genomeOffset[r];
+                    scoreLimitALT -= alt->score[r];
+                } else {
+                    alt->status[r] = SNAPGPU_NOT_FOUND;
+                }
+            }
         } else {
             result->usedAffineGapScoring[r] = 0;
             skipAffineGap[r] = true;
@@ -1010,6 +1196,7 @@ SG_HDN void sg_paired_align_ag(SgPairedAligner &P, snapgpu_paired_result *result
             result->status[w] = SNAPGPU_NOT_FOUND; result->clippingForReadAdjustment[w] = 0; result->usedAffineGapScoring[w] = 0; result->usedGaplessClipping[w] = 0;
             result->basesClippedBefore[w] = 0; result->basesClippedAfter[w] = 0; result->agScore[w] = SG_SCORE_ABOVE_LIMIT; result->seedOffset[w] = 0;
             result->lvIndels[w] = 0; result->matchProbability[w] = 0.0;
+            alt->status[w] = SNAPGPU_NOT_FOUND;
         }
         result->probabilityAllPairs = 0.0;
         return;
@@ -1019,11 +1206,22 @@ SG_HDN void sg_paired_align_ag(SgPairedAligner &P, snapgpu_paired_result *result
     nonAlt.init(P.invalidLocation);
     bool nonALTAlignment = (!pr.altAwareness) || !P.isALT(result->location[0]);
     all.initFrom(result);
+    bool altBestAlignment = false;
+    if (alt->status[0] != SNAPGPU_NOT_FOUND && alt->status[1] != SNAPGPU_NOT_FOUND) {
+        altBestAlignment = all.updateBestHitIfNeededR(alt->score[0] + alt->score[1], alt->agScore[0] + alt->agScore[1],
+                                                      alt->matchProbability[0] * alt->matchProbability[1], alt);
+    }
     if (nonALTAlignment) nonAlt.initFrom(result);
     if (!skipAffineGap[0] || !skipAffineGap[1]) {
         double newPairProbability = result->matchProbability[0] * result->matchProbability[1];
-        all.updateProbabilityOfAllPairs(oldPairProbabilityBestResult);
-        all.updateProbabilityOfBestPair(newPairProbability);
+        if (altBestAlignment) {
+            // the ALT pair's probability is in the total already (updateBestHitIfNeeded above)
+            all.updateProbabilityOfAllPairs(oldPairProbabilityBestResultALT);
+            all.updateProbabilityOfBestPair(alt->matchProbability[0] * alt->matchProbability[1], false);
+        } else {
+            all.updateProbabilityOfAllPairs(oldPairProbabilityBestResult);
+            all.updateProbabilityOfBestPair(newPairProbability);
+        }
         if (nonALTAlignment) {
             nonAlt.updateProbabilityOfAllPairs(oldPairProbabilityBestResult);
             nonAlt.updateProbabilityOfBestPair(newPairProbability);
@@ -1088,7 +1286,15 @@ SG_HDN void sg_paired_align_ag(SgPairedAligner &P, snapgpu_paired_result *result
 
     const SgPairScoreSet *emit = ((!pr.altAwareness) || nonAlt.bestPairScore > all.bestPairScore + pr.maxScoreGapToPreferNonAltAlignment) ? &all : &nonAlt;
     emit->fillInResult(T, result, result->popularSeedsSkipped);
-    (void)pp;
+    if (pr.altAwareness && emit == &nonAlt &&
+        (all.bestResultGenomeLocation[0] != nonAlt.bestResultGenomeLocation[0] || all.bestResultGenomeLocation[1] != nonAlt.bestResultGenomeLocation[1])) {
+        all.fillInResult(T, alt, alt->popularSeedsSkipped);
+        alt->supplementary[0] = alt->supplementary[1] = 1;
+    } else {
+        alt->status[0] = alt->status[1] = SNAPGPU_NOT_FOUND;
+    }
+    // without ALT contigs (projStart == NULL) nothing is ALT, the two score sets agree and there is nothing to lift over
+    if (pp.useSoftClip && pr.altAwareness && P.ix->projStart) sg_paired_alt_liftover<AGM>(P, result);
 }
 
 // (re)derive the per-read strings and pointers alignLandauVishkin sets up (:347-372), for a worker that takes a pair over at the
@@ -1121,7 +1327,9 @@ SG_HDN void sg_paired_restore_reads(SgPairedAligner &P, const uint8_t *const rea
 // ChimericPairedEndAligner::align (ChimericPairedEndAligner.cpp:126-448) around IntersectingPairedEndAligner::align (:169-252), cut in
 // two at the point where the seed / Landau-Vishkin phases (alignLandauVishkin, incl. the Hamming retry) are over and the
 // affine-gap phase and the single-end fallback begin.  What crosses the cut: `result`, the phase-4 candidate list
-// (P.ps.lvCandidates[0, nLVCand)) and the return value of stage 1.  sg_paired_align() is the two stages back to back; the
+// (P.ps.lvCandidates[0, nLVCand)) and the return value of stage 1.  When that value has SG_STAGE_ALT_RESULT set, the last record of the
+// list is the pair's firstALTResult: a launch form that hands the candidates over hands it over too, and stage 2 takes it back to its slot
+// (P.altResult()).  sg_paired_align() is the two stages back to back; the
 // device may run them in different kernels (sg_align_paired_kernel) so that each kernel's code stays small.
 //   stage 1 returns 0: `result` is final (or P.error is set); 1: continue, both reads were long enough for the paired aligner;
 //   2: continue, one read is too short (single-end fallback only).
@@ -1139,6 +1347,9 @@ SG_HDN int sg_paired_align_stage1(SgPairedAligner &P, const uint8_t *const readB
     result->agForcedSingleAlignerCall = 0;
     const uint32_t minReadLength = pr.minReadLength;
     *nLVCand = 0;
+    snapgpu_paired_result *alt = P.altResult();
+    alt->status[0] = alt->status[1] = SNAPGPU_NOT_FOUND;                   // ChimericPairedEndAligner.cpp:162
+    alt->popularSeedsSkipped[0] = alt->popularSeedsSkipped[1] = 0;
 
     if (lens[0] < minReadLength && lens[1] < minReadLength) {
         for (int w = 0; w < 2; w++) { result->location[w] = P.invalidLocation; result->mapq[w] = 0; result->score[w] = 0; result->status[w] = SNAPGPU_NOT_FOUND; }
@@ -1154,6 +1365,17 @@ SG_HDN int sg_paired_align_stage1(SgPairedAligner &P, const uint8_t *const readB
             fit = sg_paired_align_lv(P, readBases, readQuals, lens, result, nLVCand, true);
             if (!fit || P.error) { P.error = P.error ? P.error : (pp.agCandCap < SG_MAX_AG_CANDIDATES ? 4 : 2); return 0; }
         }
+        if (alt->status[0] != SNAPGPU_NOT_FOUND || alt->status[1] != SNAPGPU_NOT_FOUND || alt->popularSeedsSkipped[0] || alt->popularSeedsSkipped[1]) {
+            // the firstALTResult crosses the cut as one more candidate record (its slot follows the candidates: nLVCand <= agCandCap).  It
+            // swaps places with what that candidate slot held, and stage 2 swaps them back: candidate records keep a field the reference
+            // never writes (refSpan, see sg_paired_fill_candidate_result), so the buffer must not remember the ALT record
+            if (*nLVCand != (int)pp.agCandCap) {
+                snapgpu_paired_result &held = P.wsKey;
+                held = P.ps.lvCandidates[*nLVCand]; P.ps.lvCandidates[*nLVCand] = *alt; *alt = held;
+            }
+            (*nLVCand)++;
+            return 1 | SG_STAGE_ALT_RESULT;
+        }
         return 1;
     }
     return 2;
@@ -1167,6 +1389,18 @@ SG_HDN int sg_paired_align_stage2(SgPairedAligner &P, snapgpu_paired_result *res
 {
     const SgParams &pr = *P.pr; const SgPairedParams &pp = *P.pp;
     bool compareWithSingleEndAlignment = false;
+    snapgpu_paired_result *alt = P.altResult();
+    if (stage & SG_STAGE_ALT_RESULT) {
+        nLVCand--;
+        if (nLVCand != (int)pp.agCandCap) {
+            snapgpu_paired_result &held = P.wsKey;
+            held = P.ps.lvCandidates[nLVCand]; P.ps.lvCandidates[nLVCand] = *alt; *alt = held;
+        }
+        stage &= ~SG_STAGE_ALT_RESULT;
+    } else {
+        alt->status[0] = alt->status[1] = SNAPGPU_NOT_FOUND;
+        alt->popularSeedsSkipped[0] = alt->popularSeedsSkipped[1] = 0;
+    }
     if (stage == 1) {
         P.maxK = (int)pr.maxK;
         if (pr.useAffineGap) sg_paired_align_ag<AGM>(P, result, &nLVCand);
@@ -1178,13 +1412,20 @@ SG_HDN int sg_paired_align_stage2(SgPairedAligner &P, snapgpu_paired_result *res
         int maxScore = result->score[0] > result->score[1] ? result->score[0] : result->score[1];
         result->mapq[0] = result->mapq[0] <= pp.flattenMAPQAtOrBelow ? 0 : result->mapq[0];
         result->mapq[1] = result->mapq[1] <= pp.flattenMAPQAtOrBelow ? 0 : result->mapq[1];
-        if ((result->usedAffineGapScoring[0] || result->usedAffineGapScoring[1]) && maxScore >= pp.minScoreRealignment) compareWithSingleEndAlignment = true;
+        // an ALT pair at least minScoreGapRealignmentALT better than the result, or a lifted-over result, is not split up by the single-end
+        // aligner (ChimericPairedEndAligner.cpp:225-242)
+        const bool seenBetterAltResult = alt->status[0] != SNAPGPU_NOT_FOUND && alt->status[1] != SNAPGPU_NOT_FOUND &&
+                                         alt->score[0] + alt->score[1] <= result->score[0] + result->score[1] - pp.minScoreGapRealignmentALT;
+        const bool useAltLiftover = result->liftover[0] && result->liftover[1];
+        if ((result->usedAffineGapScoring[0] || result->usedAffineGapScoring[1]) && maxScore >= pp.minScoreRealignment && !seenBetterAltResult && !useAltLiftover)
+            compareWithSingleEndAlignment = true;
         if (result->status[0] != SNAPGPU_NOT_FOUND && result->status[1] != SNAPGPU_NOT_FOUND && !compareWithSingleEndAlignment) return 0;
     }
     return compareWithSingleEndAlignment ? 2 : 1;
 }
 
-// stage 3: ChimericPairedEndAligner.cpp:268-448, the single-end aligner on each read and the choice between its result and the pair's
+// stage 3: ChimericPairedEndAligner.cpp:268-448, the single-end aligner on each read and the choice between its result and the pair's.
+// (Its two writes to firstALTResult, :296 and :418, only decide whether -ea would write that record out, so they are not restated.)
 SG_HDN void sg_paired_align_stage3(SgPairedAligner &P, const uint8_t *const readBases[2], const uint8_t *const readQuals[2], const uint32_t lens[2],
                                    snapgpu_paired_result *result, int stage)
 {

@@ -70,6 +70,9 @@ struct snapgpu_index {
     uint32_t *d_overflow = nullptr;
     uint8_t  *d_basesPadded = nullptr;
     int64_t  *d_contigStart = nullptr;
+    int64_t  *d_projStart = nullptr;     // ALT liftover data (SgIndexView::projStart / projRC / projOps); NULL without ALT contigs
+    uint8_t  *d_projRC = nullptr;
+    uint32_t *d_projOps = nullptr;
     SgTables *d_tables_prob = nullptr;   // probability / schedule tables
     SgTables  h_tables_prob;
     // host-side metadata (needed to write the index back out in the reference's directory format)
@@ -78,6 +81,9 @@ struct snapgpu_index {
     std::vector<std::string> h_contigName;
     std::vector<uint8_t> h_contigIsAlt;
     std::vector<int32_t> h_contigOriginal;   // originalContigNumber of each contig (Genome.h:470)
+    std::vector<int64_t> h_projStart;
+    std::vector<uint8_t> h_projRC;
+    std::vector<uint32_t> h_projOps;
 };
 
 struct snapgpu_aligner {
@@ -915,12 +921,19 @@ static int upload_index(const SgHostIndex &h, int device, snapgpu_index **out)
     UP(ix->d_overflow, h.overflow.data(), h.overflow.size() * 4);          // (sg_load_index_directory leaves 8 words of slack: bulk copies round up to 16 bytes)
     UP(ix->d_basesPadded, h.basesPadded.data(), h.basesPadded.size());
     UP(ix->d_contigStart, h.contigStart.data(), h.contigStart.size() * 8);
+    if (!h.projStart.empty()) {
+        UP(ix->d_projStart, h.projStart.data(), h.projStart.size() * 8);
+        UP(ix->d_projRC, h.projRC.data(), h.projRC.size());
+        UP(ix->d_projOps, h.projOps.data(), h.projOps.size() * 4);
+        ix->h_projStart = h.projStart; ix->h_projRC = h.projRC; ix->h_projOps = h.projOps;
+    }
     sg_init_tables(ix->h_tables_prob, h.seedLen);
     UP(ix->d_tables_prob, &ix->h_tables_prob, sizeof(SgTables));
     #undef UP
     SgIndexView v = h.view();
     v.tables = ix->d_tables; v.tableStart = ix->d_tableStart; v.tableSize = ix->d_tableSize; v.tableMagic = ix->d_tableMagic; v.overflow = ix->d_overflow;
     v.bases = ix->d_basesPadded + SG_N_PADDING; v.contigStart = ix->d_contigStart;
+    v.projStart = ix->d_projStart; v.projRC = ix->d_projRC; v.projOps = ix->d_projOps;
     ix->view = v;
     memset(&ix->info, 0, sizeof(ix->info));
     ix->info.countOfBases = h.nBases; ix->info.seedLen = h.seedLen; ix->info.hashTableKeySize = h.keyBytes;
@@ -1241,10 +1254,17 @@ static int clone_alloc(const snapgpu_index *src, int device, snapgpu_index **out
     DUP(ix->d_basesPadded, src->d_basesPadded, (size_t)sv.nBases + 2 * SG_N_PADDING);
     DUP(ix->d_contigStart, src->d_contigStart, (size_t)sv.nContigs * 8);
     DUP(ix->d_tables_prob, src->d_tables_prob, sizeof(SgTables));
+    if (src->d_projStart) {
+        DUP(ix->d_projStart, src->d_projStart, src->h_projStart.size() * 8);
+        DUP(ix->d_projRC, src->d_projRC, src->h_projRC.size());
+        DUP(ix->d_projOps, src->d_projOps, src->h_projOps.size() * 4);
+    }
     #undef DUP
     SgIndexView v = sv;
     v.tables = ix->d_tables; v.tableStart = ix->d_tableStart; v.tableSize = ix->d_tableSize; v.tableMagic = ix->d_tableMagic; v.overflow = ix->d_overflow;
     v.bases = ix->d_basesPadded + SG_N_PADDING; v.contigStart = ix->d_contigStart; v.buckets = ix->d_buckets;
+    v.projStart = ix->d_projStart; v.projRC = ix->d_projRC; v.projOps = ix->d_projOps;
+    ix->h_projStart = src->h_projStart; ix->h_projRC = src->h_projRC; ix->h_projOps = src->h_projOps;
     ix->view = v;
     ix->builtOnDevice = src->builtOnDevice;
     ix->info = src->info; ix->info.hbmBytes = hbm;
@@ -1434,6 +1454,7 @@ void snapgpu_index_close(snapgpu_index *ix)
     cudaSetDevice(ix->device);
     cudaFree(ix->d_tables); cudaFree(ix->d_buckets); cudaFree(ix->d_tableStart); cudaFree(ix->d_tableSize); cudaFree(ix->d_tableMagic); cudaFree(ix->d_overflow);
     cudaFree(ix->d_basesPadded); cudaFree(ix->d_contigStart); cudaFree(ix->d_tables_prob);
+    cudaFree(ix->d_projStart); cudaFree(ix->d_projRC); cudaFree(ix->d_projOps);
     delete ix;
 }
 
@@ -1701,10 +1722,6 @@ int snapgpu_paired_aligner_create(const snapgpu_index *idx, const snapgpu_params
     *out = nullptr;
     if (require_device(idx->device)) return 1;
     if (maxBatchPairs <= 0) return sg_fail("maxBatchPairs must be positive");
-    // ALT-aware pairing (a second score set for non-ALT pairs, ALT liftover) is not implemented; with ALT awareness off (-ea-) an index with ALT contigs
-    // is just an index, and results are the reference's (host build: 8 option sets x 2 pair sets on an ALT-bearing reference)
-    if (idx->view.altFirstLocation < idx->view.nBases && params->altAwareness)
-        return sg_fail("snapgpu_paired_aligner_create: ALT-aware pairing is not supported: an index with ALT contigs needs -ea- (altAwareness = 0) on the paired path");
     snapgpu_aligner *a = new (std::nothrow) snapgpu_aligner;
     if (!a) return sg_fail("out of memory");
     a->index = idx; a->device = idx->device; a->userParams = *params; a->maxBatchReads = 2 * maxBatchPairs; a->paired = true;
