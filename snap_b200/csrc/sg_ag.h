@@ -29,6 +29,8 @@ SG_HD SgAgParams sg_ag_params(int matchReward, int subPenalty, int gapOpen, int 
 // The specialised device forms (packed s16x2 rows, narrow-band rows) do plain 16-bit arithmetic where the reference saturates, and
 // the packed one pads with -16384 instead of INT16_MIN.  That is exact as long as no cell value can come near either: true for any
 // sane scoring scheme, checked here so that an exotic one falls back to the general form (which saturates like the reference).
+// The guard is about saturation only: every form keeps the query profile at full int16 width, so any match reward or substitution
+// penalty is represented exactly.  tests/test_scoring_schemes.py pins which side of it each tested scheme falls on.
 SG_HD bool sg_ag_small_scores(const SgAgParams &P, uint32_t maxReadLen)
 {
     const long long top = (long long)(P.matchReward > 0 ? P.matchReward : 0) * ((long long)maxReadLen + SG_MAX_K + 1)

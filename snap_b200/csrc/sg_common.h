@@ -132,7 +132,8 @@ struct SgScratch {
     // affine gap
     int16_t  *agH, *agHm1, *agE;     // [agCols]
     uint8_t  *agBt[2];               // [agRows*agCols] traceback bits; [0] forward object, [1] reverse object; PERSISTENT across calls
-    int8_t   *agProf;                // [10*agCols bytes] striped query profile of the current affine-gap call (device warp form)
+    int16_t  *agProf;                // [5*agCols] striped query profile of the current affine-gap call (device warp forms): int16 per cell in
+                                     // every form, as the reference keeps it (the packed forms pair two cells as s16x2)
     uint32_t agCols, agRows;
     uint32_t *agSnap;                // [7*32] H after each lazy-F round of the experimental narrow-band form (sg_warp_ag_duo.cuh): shared memory
                                      // where the kernel has a block for it, NULL = the Landau-Vishkin cell array of the arena (idle during an affine-gap call)
@@ -166,7 +167,7 @@ SG_HD size_t sg_scratch_bytes(const SgParams &p)
     b += sg_align_up(SG_MAX_K + 2, 256);
     b += sg_align_up(sizeof(int16_t) * agCols, 256) * 3;
     b += sg_align_up(agRows * agCols, 256) * 2;
-    b += sg_align_up(10 * agCols, 256);               // (two bytes per column: the packed forms keep the profile as s16x2)
+    b += sg_align_up(10 * agCols, 256);               // agProf: five int16 rows of up to agCols cells
     return b;
 }
 
@@ -192,7 +193,7 @@ SG_HD void sg_scratch_carve(const SgParams &p, uint8_t *base, SgScratch *s)
     s->agE = (int16_t *)q;            q += sg_align_up(sizeof(int16_t) * agCols, 256);
     s->agBt[0] = q;                   q += sg_align_up(agRows * agCols, 256);
     s->agBt[1] = q;                   q += sg_align_up(agRows * agCols, 256);
-    s->agProf = (int8_t *)q;          q += sg_align_up(10 * agCols, 256);
+    s->agProf = (int16_t *)q;         q += sg_align_up(10 * agCols, 256);
     s->agCols = (uint32_t)agCols;
     s->agRows = (uint32_t)agRows;
     s->agSnap = (uint32_t *)0;

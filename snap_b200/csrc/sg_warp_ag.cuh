@@ -32,7 +32,7 @@ __device__ __noinline__ void sg_warp_ag_rows_banded4(const SgScratch &S, int ope
     const int stride = lay.rowStride();
     const int l = lane & 7, q = lane >> 3;
     int16_t *Hptr = S.agH, *Hm1ptr = S.agHm1, *E = S.agE;
-    const int8_t *prof = S.agProf;
+    const int16_t *prof = S.agProf;
     int bestG = -1, bestGT = -1, bestL = -1, bestLT = -1, bestLP = -1;
     const int globalIdx = lay.cellIndex(patternLen - 1);
     int segBegTrack = 0, segEndTrack = ((w < patternLen - 1) ? w : (patternLen - 1)) / segLen;
@@ -42,7 +42,7 @@ __device__ __noinline__ void sg_warp_ag_rows_banded4(const SgScratch &S, int ope
     for (int i = 0; i < textLen; i++) {
         const uint32_t tb = sg_base_value(text[i * dir]);
         uint8_t *btRow = bt + (size_t)i * stride;
-        const int8_t *profRow = prof + tb * stride;
+        const int16_t *profRow = prof + tb * stride;
         int myMax = 0, myMaxCol = -1, X0 = 0;
         const int bandBeg = (i - w) > 0 ? (i - w) : 0;
         const int bandEnd = (i + w) < (patternLen - 1) ? (i + w) : (patternLen - 1);
@@ -71,7 +71,7 @@ __device__ __noinline__ void sg_warp_ag_rows_banded4(const SgScratch &S, int ope
                 if (q == 0) hdiag = (l == 0) ? hInit : (int)Hptr[(vbase + numVec - 1) * SG_VEC + l - 1];
                 else hdiag = Hptr[idx - SG_VEC];
                 const int pv = profRow[idx];
-                const int m = (hdiag > 0) ? hdiag + (pv == -128 ? -32768 : pv) : 0;      // (no saturation can occur here: sg_ag_small_scores)
+                const int m = (hdiag > 0) ? hdiag + pv : 0;      // (no saturation can occur here: sg_ag_small_scores)
                 const int e = E[idx];
                 act = (e > m) ? 1 : 0;
                 h = m > e ? m : e;
@@ -103,6 +103,7 @@ __device__ __noinline__ void sg_warp_ag_rows_banded4(const SgScratch &S, int ope
             const unsigned stopBits = 0x80808080u & (nVecHere >= 4 ? 0xffffffffu : ((1u << (8 * nVecHere)) - 1u));
             const unsigned beforeMe = 0x80808080u & ((1u << (8 * q)) - 1u);
             const int dRound = nVecHere * ext, fl0 = fl;
+            // 0x3fff beats every F: F is a decayed cell value, and sg_ag_small_scores keeps cell values below 12000 for this form
             if (!valid) h = 0x3fff;
             int nRounds = 0;
             #pragma unroll 1
@@ -239,13 +240,14 @@ __device__ __noinline__ void sg_warp_ag_compute(const SgTables &T, const SgScrat
                      bb.lScore, bb.lText, bb.lPat, bb.gScore, bb.gText, out);
         return;
     }
-    // striped query profile (the reference's qProfile, :921-935 / :348-365) as int8, -128 standing for the INT16_MIN padding
-    int8_t *prof = S.agProf;
+    // striped query profile (the reference's qProfile, :921-935 / :348-365) as int16 with the reference's INT16_MIN padding: any
+    // match reward or substitution penalty of the scheme fits
+    int16_t *prof = S.agProf;
     for (int idx = lane; idx < stride; idx += 32) {
         const int vec = idx >> 3, ll = idx & 7;
         const int col = (vec / numVec) * segLen + ll * numVec + (vec % numVec);
         const uint32_t pb = (col < patternLen) ? sg_base_value(pattern[col]) : 5u;
-        for (uint32_t t = 0; t < 5; t++) prof[t * stride + idx] = (pb == 5u) ? (int8_t)-128 : (int8_t)sg_ag_sub(P, t, pb);
+        for (uint32_t t = 0; t < 5; t++) prof[t * stride + idx] = (pb == 5u) ? (int16_t)-32768 : (int16_t)sg_ag_sub(P, t, pb);
     }
     __syncwarp();
 
@@ -268,7 +270,7 @@ __device__ __noinline__ void sg_warp_ag_compute(const SgTables &T, const SgScrat
         lay.nRows = i + 1;
         const uint32_t tb = sg_base_value(text[i * dir]);
         uint8_t *btRow = bt + (size_t)i * stride;
-        const int8_t *profRow = prof + tb * stride;
+        const int16_t *profRow = prof + tb * stride;
         int myMax = 0;                   // running max of H over the cells this lane committed in this row
         int myMaxCol = -1;               // ... and the largest column at which this lane saw it
         int X0 = 0;                      // lane 0 of the reference's X register
@@ -318,7 +320,7 @@ __device__ __noinline__ void sg_warp_ag_compute(const SgTables &T, const SgScrat
                     if (k == 0) hdiag = (l == 0) ? hInit : (int)Hptr[(vbase + numVec - 1) * SG_VEC + l - 1];
                     else hdiag = Hptr[idx - SG_VEC];
                     const int pv = profRow[idx];
-                    const int m = (hdiag > 0) ? sg_sat16(hdiag + (pv == -128 ? -32768 : pv)) : 0;
+                    const int m = (hdiag > 0) ? sg_sat16(hdiag + pv) : 0;
                     const int e = E[idx];
                     act = (e > m) ? 1 : 0;
                     h = m > e ? m : e;
@@ -383,7 +385,7 @@ __device__ __noinline__ void sg_warp_ag_compute(const SgTables &T, const SgScrat
                     if (k == 0) hdiag = (l == 0) ? hInit : (int)Hptr[(vbase + numVec - 1) * SG_VEC + l - 1];
                     else hdiag = Hptr[idx - SG_VEC];
                     const int pv = profRow[idx];
-                    const int m = (hdiag > 0) ? sg_sat16(hdiag + (pv == -128 ? -32768 : pv)) : 0;
+                    const int m = (hdiag > 0) ? sg_sat16(hdiag + pv) : 0;
                     const int e = E[idx];
                     act = (e > m) ? 1 : 0;
                     h1 = m > e ? m : e;

@@ -138,7 +138,17 @@ static void make_scratch(const SgParams &p, std::vector<uint8_t> &mem, SgScratch
     sg_scratch_carve(p, base, s);
 }
 
+static const uint32_t WS_MAX_READ_LEN = 1000;         // the scratch of the emulated warp, like the device leaf tests' (leaf_scratch)
+
 extern "C" {
+
+// sg_ag_small_scores for a scoring scheme (the reference's order: match, sub, open, extend, 5', 3'), at the emulated warp's maxReadLen:
+// whether the alignment kernels would take the specialised forms (packed rows, narrow-band rows) under it.
+int ws_ag_small_scores(const snapgpu_ag_params *ap)
+{
+    SgAgParams P = sg_ag_params(ap->matchReward, ap->subPenalty, ap->gapOpenPenalty, ap->gapExtendPenalty, ap->fivePrimeEndBonus, ap->threePrimeEndBonus);
+    return sg_ag_small_scores(P, WS_MAX_READ_LEN) ? 1 : 0;
+}
 
 // Same contract as hostsim's hs_ag_batch / the ABI's snapgpu_test_ag_warp: one emulated warp runs the jobs in order (so the
 // traceback array carries over from job to job like the reference's).  usePacked: SgAgParams.usePacked (0 int forms, 1 packed, 2 unrolled packed;
@@ -149,7 +159,7 @@ long long ws_ag_batch(const snapgpu_ag_params *ap, const char *textBuf, const ch
     static SgTables T; static bool init = false;
     if (!init) { sg_init_tables(T, 20); init = true; }
     SgParams p; memset(&p, 0, sizeof(p));
-    p.poolSize = 1; p.tableSlots = 2; p.numWeightLists = 2; p.maxReadLen = 1000;
+    p.poolSize = 1; p.tableSlots = 2; p.numWeightLists = 2; p.maxReadLen = WS_MAX_READ_LEN;
     std::vector<uint8_t> mem; SgScratch s; make_scratch(p, mem, &s);
     static SgWarpSmall small;                    // the per-warp shared-memory block of the alignment kernels
     if (usePacked & 8) { usePacked &= ~8; }      // 8: without it (the arena copies are used, as in the leaf test kernel)

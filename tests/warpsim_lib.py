@@ -38,6 +38,8 @@ def lib():
         L = C.CDLL(build())
         L.ws_ag_batch.restype = C.c_longlong
         L.ws_ag_batch.argtypes = [C.c_void_p] * 5 + [C.c_int64, C.c_void_p, C.c_int]
+        L.ws_ag_small_scores.restype = C.c_int
+        L.ws_ag_small_scores.argtypes = [C.c_void_p]
         _lib = L
     return _lib
 
@@ -51,3 +53,10 @@ def ag_batch(text, pat, qual, jobs, out_dtype, params, packed=1):
     params = np.ascontiguousarray(params, dtype=np.int32)
     lib().ws_ag_batch(_p(params), _p(text), _p(pat), _p(qual), _p(np.ascontiguousarray(jobs)), jobs.size, _p(out), packed)
     return out
+
+
+def small_scores(params) -> bool:
+    """sg_ag_small_scores (snap_b200/csrc/sg_ag.h) for a scheme [match, sub, open, extend, 5' bonus, 3' bonus] at maxReadLen 1000 (the
+    leaf tests' scratch): True when the kernels may take the specialised affine-gap forms under it."""
+    params = np.ascontiguousarray(params, dtype=np.int32)
+    return bool(lib().ws_ag_small_scores(_p(params)))
