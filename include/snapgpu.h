@@ -202,6 +202,10 @@ int  snapgpu_index_open(const char *directory, int device, snapgpu_index **out);
  * Equivalent in *results* to GenomeIndex::BuildIndexToDirectory (GenomeIndex.cpp:527-1110): every
  * seed maps to the same hit set in the same (descending) order; slot layout is not part of the contract.
  * contigStarts[nContigs] are the beginningLocation values (first real base of each contig).
+ * Memory: beside the finished index (bases, buckets or tables, overflow table), one sweep sorts every position at once in
+ * 24 bytes each (~72 GB at 3 Gbp).  When that, or the 12 bytes per position it keeps while the index is allocated, does not fit
+ * the free device memory, the build sorts the positions in key-range passes that each fit (SNAPGPU_BUILD_PASSES=n asks for at
+ * least n); a 3 Gbp bucket index then builds on an 80 GB device.  The index is the same either way.
  */
 int  snapgpu_index_build(const char *bases, int64_t nBases, const int64_t *contigStarts, uint32_t nContigs,
                          uint32_t seedLen, uint32_t chromosomePadding, int device, snapgpu_index **out);
@@ -209,7 +213,9 @@ int  snapgpu_index_build(const char *bases, int64_t nBases, const int64_t *conti
 int  snapgpu_index_build_device(const char *d_bases, int64_t nBases, const int64_t *contigStarts, uint32_t nContigs,
                                 uint32_t seedLen, uint32_t chromosomePadding, int device, snapgpu_index **out);
 /* Writes the HBM-resident index out as a reference-format directory (the four files `snap-aligner index` produces,
- * SURVEY 8a-F) so stock SNAP can load an index built on the device. */
+ * SURVEY 8a-F) so stock SNAP can load an index built on the device.  A device-built bucket index has its buckets re-laid into
+ * the reference's tables one range of tables at a time, in a buffer of at most the free device memory (8 bytes per table slot,
+ * ~1.3 x the distinct seeds; SNAPGPU_BUILD_PASSES=n: at least n ranges).  Seed length 16 has a single table, which must fit whole. */
 int  snapgpu_index_save(const snapgpu_index *idx, const char *directory);
 int  snapgpu_index_info_get(const snapgpu_index *idx, snapgpu_index_info *info);
 /*

@@ -47,6 +47,29 @@ SG_HD uint64_t sg_bucket_mix(uint64_t c, uint32_t bits)
     return x;
 }
 
+// Inverse of an odd multiplier mod 2^64 (Newton: each step doubles the correct low bits, 3 -> 96).
+SG_HD uint64_t sg_odd_inverse(uint64_t m)
+{
+    uint64_t x = m;                                            // m * m == 1 mod 8
+    for (int i = 0; i < 5; i++) x *= 2 - m * x;
+    return x;
+}
+
+// Inverse of sg_bucket_mix: the xor-shifts by bits/2 undo themselves on a bits-wide value, the multiplications by the inverses.
+SG_HD uint64_t sg_bucket_unmix(uint64_t h, uint32_t bits)
+{
+    const uint64_t mask = (bits >= 64) ? ~0ULL : ((1ULL << bits) - 1);
+    const uint32_t s = bits / 2;
+    uint64_t x = h & mask;
+    x ^= x >> s;
+    x = (x * sg_odd_inverse(0x9e3779b97f4a7c15ULL)) & mask;
+    x ^= x >> s;
+    x = (x * sg_odd_inverse(0xc4ceb9fe1a85ec53ULL)) & mask;
+    x ^= x >> s;
+    x = (x * sg_odd_inverse(0xff51afd7ed558ccdULL)) & mask;
+    return x;
+}
+
 SG_HD uint64_t sg_mulhi64(uint64_t a, uint64_t b)
 {
 #if defined(__CUDA_ARCH__)
@@ -72,6 +95,33 @@ SG_HD uint64_t sg_bucket_min_count(uint32_t bits)
 SG_HD uint64_t sg_bucket_slot_make(uint64_t h, uint32_t orient, uint32_t value)
 {
     return ((uint64_t)orient << 62) | ((h & 0x3fffffffULL) << 32) | value;
+}
+
+SG_HD uint64_t sg_seed_revcomp(uint64_t bases, uint32_t seedLen);      // sg_seed.h
+
+// The seed whose locations a used slot of bucket b holds (the canonical seed, or its reverse complement for orientation 1).  The
+// hidden high bits of h: the key's home is b or up to SG_BUCKET_MAX_DISP buckets before it (wrapping at bucket 0), and homes of
+// h values that differ in their high bits lie >= 2 * (SG_BUCKET_MAX_DISP + 1) buckets apart, so of the largest high part whose
+// homes start at or before b and the one below it, exactly one places the key within reach.  False if neither does.
+SG_HD bool sg_bucket_slot_decode(uint64_t slot, uint64_t b, uint64_t nBuckets, uint32_t seedLen, uint64_t *seed, uint32_t *orient)
+{
+    const uint32_t bits = 2 * seedLen, hidden = bits - 30;
+    const uint64_t tag = (slot >> 32) & 0x3fffffffULL, nHigh = 1ULL << hidden;
+    // largest hi with floor(hi * nBuckets / 2^hidden) <= b, i.e. hi * nBuckets < (b + 1) * 2^hidden
+    const uint64_t top = (((b + 1) << hidden) + nBuckets - 1) / nBuckets - 1;
+    for (int k = 0; k < 2; k++) {
+        const uint64_t hi = (top + nHigh - (uint64_t)k) & (nHigh - 1);
+        const uint64_t h = (hi << 30) | tag;
+        const uint64_t home = sg_bucket_home(h, bits, nBuckets);
+        const uint64_t disp = b >= home ? b - home : b + nBuckets - home;
+        if (disp <= SG_BUCKET_MAX_DISP) {
+            const uint64_t c = sg_bucket_unmix(h, bits);
+            *orient = (uint32_t)((slot >> 62) & 1);
+            *seed = *orient ? sg_seed_revcomp(c, seedLen) : c;
+            return true;
+        }
+    }
+    return false;
 }
 
 // The four slots of bucket b, one sector.

@@ -9,9 +9,13 @@
 //
 // Method: emit (seed, location) for locations in descending order, stable LSD radix sort on the seed (so equal
 // seeds keep descending locations), then one pass sizes the tables and one pass inserts run heads with atomicCAS
-// along the very probe sequence lookups use.
+// along the very probe sequence lookups use.  When the sort scratch (24 bytes per position) does not fit the device at once, the
+// builder runs the same sort / count / insert in passes over ranges of the seed's top 16 bits, each pass selecting its own
+// positions in the same descending order (snapgpu.cu build_index_on_device).
 #pragma once
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_select.cuh>
+#include <thrust/iterator/counting_iterator.h>
 
 
 __global__ void sg_build_emit_kernel(const uint8_t *bases /* location 0 */, long long nPositions, uint32_t seedLen,
@@ -150,6 +154,19 @@ __global__ void sg_build_count_values_kernel(const uint8_t *tables, unsigned lon
     if ((threadIdx.x & 31) == 0 && local) atomicAdd(count, local);
 }
 
+// Places (key, value) in one of the reference's tables along SNAPHashTable's probe sequence; false if the table is full.
+__device__ __forceinline__ bool sg_table_insert_atomic(unsigned long long *table, uint64_t size, unsigned long long low, uint32_t value)
+{
+    const unsigned long long EMPTY = 0x00000000ffffffffULL;   // key 0, value invalid (HashTable.cpp:66-72)
+    const unsigned long long entry = (low << 32) | value;
+    uint64_t idx = sg_fmix64(low) % size;
+    for (unsigned long long nProbes = 0;;) {
+        if (atomicCAS(&table[idx], EMPTY, entry) == EMPTY) return true;
+        if (++nProbes > size + 5) return false;
+        idx = sg_table_probe_next(idx, nProbes, size);
+    }
+}
+
 // pass 2: insert run heads.  buckets != NULL: into sector buckets (sg_bucket.h); else into the reference's table layout.
 __global__ void sg_build_insert_kernel(const unsigned long long *keys, const uint32_t *locs, long long n, uint32_t keyBits, uint32_t seedLen,
                                        const uint64_t *tableStart, const uint64_t *tableSize, unsigned long long *tables,
@@ -158,7 +175,6 @@ __global__ void sg_build_insert_kernel(const unsigned long long *keys, const uin
 {
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long stride = (long long)gridDim.x * blockDim.x;
-    const unsigned long long EMPTY = 0x00000000ffffffffULL;   // key 0, value invalid (HashTable.cpp:66-72)
     const unsigned long long SG_BUILD_INVALID_KEY = 1ULL << (2 * seedLen);
     for (; i < n; i += stride) {
         unsigned long long k = keys[i];
@@ -183,20 +199,85 @@ __global__ void sg_build_insert_kernel(const unsigned long long *keys, const uin
             continue;
         }
         const uint32_t table = (uint32_t)(k >> keyBits);
-        const unsigned long long low = k & ((1ULL << keyBits) - 1);
-        const uint64_t size = tableSize[table], base = tableStart[table];
-        uint64_t idx = sg_fmix64(low) % size;
-        const unsigned long long entry = (low << 32) | value;
-        unsigned long long nProbes = 0;
-        bool placed = false;
-        for (;;) {
-            unsigned long long old = atomicCAS(&tables[base + idx], EMPTY, entry);
-            if (old == EMPTY) { placed = true; break; }
-            nProbes++;
-            if (nProbes > size + 5) break;
-            if (nProbes < 5) idx = (idx + nProbes * nProbes) % size; else idx = (idx + 1) % size;
-        }
-        if (!placed) *failed = 1;
+        if (!sg_table_insert_atomic(tables + tableStart[table], tableSize[table], k & ((1ULL << keyBits) - 1), value)) *failed = 1;
+    }
+}
+
+// ---- key-range passes (a build whose sort scratch does not fit at once; snapgpu.cu build_index_on_device) ----
+// A pass takes the valid seeds whose top 16 bits (the bin) lie in [binLo, binHi): all locations of a seed fall in one pass.
+
+#define SG_BUILD_BINS 65536u
+
+// the forward seed at loc, false if its bases are not all ACGT
+__device__ __forceinline__ bool sg_build_seed_at(const uint8_t *bases, long long loc, uint32_t seedLen, unsigned long long *seed)
+{
+    unsigned long long b = 0;
+    bool ok = true;
+    for (uint32_t i = 0; i < seedLen; i++) {
+        const uint32_t v = sg_base_value(bases[loc + i]);
+        ok = ok && v < 4;
+        b = (b << 2) | (v & 3);
+    }
+    *seed = b;
+    return ok;
+}
+
+// valid seeds per bin, over all positions
+__global__ void sg_build_histogram_kernel(const uint8_t *bases, long long nPositions, uint32_t seedLen, unsigned long long *bins)
+{
+    const uint32_t shift = 2 * seedLen - 16;
+    long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (; j < nPositions; j += stride) {
+        unsigned long long s;
+        if (sg_build_seed_at(bases, j, seedLen, &s)) atomicAdd(&bins[s >> shift], 1ULL);
+    }
+}
+
+// Selection predicate over j = nPositions - 1 - location (descending locations, as sg_build_emit_kernel orders them).
+struct SgBuildPassSelect {
+    const uint8_t *bases;
+    long long nPositions;
+    uint32_t seedLen, binLo, binHi;
+    __device__ __forceinline__ bool operator()(uint32_t j) const
+    {
+        unsigned long long s;
+        if (!sg_build_seed_at(bases, nPositions - 1 - (long long)j, seedLen, &s)) return false;
+        const uint32_t bin = (uint32_t)(s >> (2 * seedLen - 16));
+        return bin >= binLo && bin < binHi;
+    }
+};
+
+// the selected j (in order) -> (seed, location) pairs for the sort
+__global__ void sg_build_pass_keys_kernel(const uint8_t *bases, long long nPositions, uint32_t seedLen, long long n, uint32_t *locs, unsigned long long *keys)
+{
+    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (; i < n; i += stride) {
+        const long long loc = nPositions - 1 - (long long)locs[i];
+        unsigned long long s;
+        sg_build_seed_at(bases, loc, seedLen, &s);
+        keys[i] = s;
+        locs[i] = (uint32_t)loc;
+    }
+}
+
+// ---- saving a bucket index in the reference's layout (snapgpu_index_save), one range of tables per pass ----
+// Every used bucket slot becomes the entry (seed, value) of its table, its value unchanged (a location, or countOfBases + an
+// offset into the index's own overflow table).  tables: the range's tables back to back, table t at tableStart[t] - rangeBase.
+__global__ void sg_build_tables_from_buckets_kernel(const unsigned long long *buckets, unsigned long long nBuckets, uint32_t seedLen,
+                                                    uint32_t tableLo, uint32_t tableHi, const uint64_t *tableStart, const uint64_t *tableSize,
+                                                    uint64_t rangeBase, unsigned long long *tables, int *failed)
+{
+    const unsigned long long nSlots = nBuckets * SG_BUCKET_SLOTS;
+    for (unsigned long long s = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; s < nSlots; s += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long slot = buckets[s];
+        if ((uint32_t)slot == 0xffffffffu) continue;
+        uint64_t seed; uint32_t orient;
+        if (!sg_bucket_slot_decode(slot, s / SG_BUCKET_SLOTS, nBuckets, seedLen, &seed, &orient)) { *failed = 1; continue; }
+        const uint32_t t = (uint32_t)(seed >> 32);
+        if (t < tableLo || t >= tableHi) continue;
+        if (!sg_table_insert_atomic(tables + (tableStart[t] - rangeBase), tableSize[t], seed & 0xffffffffULL, (uint32_t)slot)) *failed = 1;
     }
 }
 

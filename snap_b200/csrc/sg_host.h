@@ -266,6 +266,70 @@ static inline bool sg_host_relayout(SgHostIndex &ix, double load, std::string &e
     return false;
 }
 
+// Writes the reference's tables (tableStart / tableSize / invalidValue as they stand) from the sector buckets: every used slot
+// becomes one (seed, value) entry, placed along SNAPHashTable's probe sequence.  The sequential form of what snapgpu_index_save
+// does on the device for an index built there; the host-side tests use it.  Recomputes tableUsed; afterwards view() hands out
+// the tables.
+static inline bool sg_host_buckets_to_tables(SgHostIndex &ix, std::string &err)
+{
+    if (ix.layout != SG_LAYOUT_BUCKET || ix.large || ix.entryBytes != 8 || ix.keyBytes != 4) { err = "buckets -> tables needs a bucket-layout index with 8-byte entries"; return false; }
+    const uint32_t keyBits = 32;
+    const uint64_t empty = (uint64_t)ix.invalidValue;                    // key 0, value invalid
+    std::vector<uint64_t> t64((size_t)ix.totalSlots + 2, empty);
+    ix.tableUsed.assign(ix.nTables, 0);
+    for (uint64_t s = 0; s < ix.nBuckets * SG_BUCKET_SLOTS; s++) {
+        const uint64_t slot = ix.buckets[s];
+        if ((uint32_t)slot == 0xffffffffu) continue;
+        uint64_t seed; uint32_t orient;
+        if (!sg_bucket_slot_decode(slot, s / SG_BUCKET_SLOTS, ix.nBuckets, ix.seedLen, &seed, &orient)) { err = "a bucket slot is out of reach of its home"; return false; }
+        const uint32_t t = (uint32_t)(seed >> keyBits);
+        const uint64_t low = seed & 0xffffffffULL, size = ix.tableSize[t], base = ix.tableStart[t];
+        uint64_t idx = sg_fmix64(low) % size, nProbes = 0;
+        while (t64[base + idx] != empty) {
+            if (++nProbes > size + 5) { err = "hash table overflow"; return false; }
+            idx = sg_table_probe_next(idx, nProbes, size);
+        }
+        t64[base + idx] = (low << 32) | (uint32_t)slot;
+        ix.tableUsed[t]++;
+    }
+    ix.tables.assign((size_t)ix.totalSlots * 8 + 16, 0);
+    memcpy(ix.tables.data(), t64.data(), (size_t)ix.totalSlots * 8);
+    ix.layout = SG_LAYOUT_SNAP;
+    ix.buckets.clear(); ix.nBuckets = 0;
+    return true;
+}
+
+// Splits bins [0, nBins) into contiguous ranges (passes) whose bytes each fit `budget`: at least minPasses of them, or one per
+// non-empty bin if there are fewer, and as few as that allows otherwise (one when everything fits).  bounds gets the P + 1 range
+// edges.  False, with *badBin, when one bin alone exceeds the budget.
+static inline bool sg_plan_passes(const uint64_t *binBytes, uint32_t nBins, uint64_t budget, uint32_t minPasses, std::vector<uint32_t> &bounds, uint32_t *badBin)
+{
+    uint64_t total = 0, nonEmptyLeft = 0;
+    for (uint32_t b = 0; b < nBins; b++) {
+        if (binBytes[b] > budget) { *badBin = b; return false; }
+        total += binBytes[b];
+        nonEmptyLeft += binBytes[b] > 0;
+    }
+    if (minPasses < 1) minPasses = 1;
+    uint64_t cap = total / minPasses;                          // forcing P passes: spread the bytes evenly
+    if (cap < 1) cap = 1;
+    if (cap > budget) cap = budget;
+    bounds.assign(1, 0);
+    uint64_t cur = 0, curNonEmpty = 0;
+    for (uint32_t b = 0; b < nBins; b++) {
+        const uint64_t w = binBytes[b];
+        if (w == 0) continue;
+        const uint64_t passesAfterThis = minPasses > bounds.size() ? minPasses - bounds.size() : 0;
+        if (curNonEmpty > 0 && (cur + w > cap || nonEmptyLeft <= passesAfterThis)) {
+            bounds.push_back(b);
+            cur = 0; curNonEmpty = 0;
+        }
+        cur += w; curNonEmpty++; nonEmptyLeft--;
+    }
+    bounds.push_back(nBins);
+    return true;
+}
+
 // ---- probability tables (reference LandauVishkin.cpp:715-763), MAPQ thresholds (mapq.h:54), wrap table ----
 
 // SeedSequencer::SeedSequencer (reference SeedSequencer.cpp:36-103): breadth-first midpoint order; the table is

@@ -61,6 +61,13 @@ SG_HD uint64_t sg_fmix64(uint64_t key)
     return key;
 }
 
+// SNAPHashTable's probe sequence (HashTable.h:87-118): quadratic for nProbes 1..4, then linear -- the sequence sg_probe walks.
+// Every insertion into the reference's table layout (sg_build.cuh, sg_host_buckets_to_tables) takes its steps from here.
+SG_HD uint64_t sg_table_probe_next(uint64_t idx, uint64_t nProbes, uint64_t size)
+{
+    return nProbes < 5 ? (idx + nProbes * nProbes) % size : (idx + 1) % size;
+}
+
 // Little-endian load of n (<=8) bytes from a possibly unaligned address.
 SG_HD uint64_t sg_load_le(const uint8_t *p, uint32_t n)
 {

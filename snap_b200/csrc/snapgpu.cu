@@ -15,6 +15,7 @@
 #include <string>
 #include <vector>
 #include <algorithm>
+#include <functional>
 #include <new>
 
 #define SG_WITH_PAIRED 1
@@ -65,7 +66,7 @@ struct snapgpu_index {
     snapgpu_index_info info;
     uint8_t  *d_tables = nullptr;        // the reference's table layout (SG_LAYOUT_SNAP); NULL for a sector-bucket index
     uint64_t *d_buckets = nullptr;       // sector buckets (SG_LAYOUT_BUCKET, sg_bucket.h)
-    bool builtOnDevice = false;          // bases -> index on the device (such an index can be re-built in the reference's layout for saving)
+    bool builtOnDevice = false;          // bases -> index on the device (its buckets are re-laid into the reference's tables for saving)
     uint64_t *d_tableStart = nullptr, *d_tableSize = nullptr, *d_tableMagic = nullptr;
     uint32_t *d_overflow = nullptr;
     uint8_t  *d_basesPadded = nullptr;
@@ -962,8 +963,113 @@ int snapgpu_index_open(const char *directory, int device, snapgpu_index **out)
     return upload_index(h, device, out);
 }
 
+// Device memory a build or save may plan with: what cudaMemGetInfo reports as free, less a margin for the allocator and the
+// driver (256 MiB + 1/64 of the device).
+static int sg_usable_bytes(size_t *out)
+{
+    size_t freeBytes = 0, totalBytes = 0;
+    SG_CUDA(cudaMemGetInfo(&freeBytes, &totalBytes));
+    const size_t margin = ((size_t)256 << 20) + totalBytes / 64;
+    *out = freeBytes > margin ? freeBytes - margin : 0;
+    return 0;
+}
+
+// SNAPGPU_BUILD_PASSES=n: the device build and the save use at least n passes (default: as few as the free memory allows).
+static uint32_t sg_min_passes()
+{
+    if (const char *e = getenv("SNAPGPU_BUILD_PASSES")) {
+        const long long v = atoll(e);
+        if (v > 1) return v > (long long)SG_BUILD_BINS ? SG_BUILD_BINS : (uint32_t)v;
+    }
+    return 1;
+}
+
+// Scratch of the key-range passes: keys and locations, double-buffered for the radix sort, and cub's storage.
+struct SgPassScratch {
+    unsigned long long *keys[2] = {nullptr, nullptr};
+    uint32_t *locs[2] = {nullptr, nullptr};
+    void *temp = nullptr;
+    long long *nSel = nullptr;
+    ~SgPassScratch() { cudaFree(keys[0]); cudaFree(keys[1]); cudaFree(locs[0]); cudaFree(locs[1]); cudaFree(temp); cudaFree(nSel); }
+};
+
+// cub storage of a pass over up to n positions (the selection runs over all nPos positions)
+static int sg_pass_temp_bytes(long long nPos, long long n, uint32_t seedLen, size_t *bytes)
+{
+    size_t sel = 0, sort = 0;
+    SgBuildPassSelect pred = {nullptr, nPos, seedLen, 0, 0};
+    SG_CUDA(cub::DeviceSelect::If(nullptr, sel, thrust::make_counting_iterator<long long>(0), (uint32_t *)nullptr, (long long *)nullptr, nPos, pred));
+    cub::DoubleBuffer<unsigned long long> kb(nullptr, nullptr);
+    cub::DoubleBuffer<uint32_t> vb(nullptr, nullptr);
+    SG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort, kb, vb, n, 0, (int)(2 * seedLen)));
+    *bytes = std::max(sel, sort) + 16;
+    return 0;
+}
+
+// Plans the key-range passes from the valid seeds per bin: 24 bytes per position of a pass, plus cub's storage, must fit the memory
+// free now.  bounds: bin edges of the passes; *maxN: positions of the largest pass.
+static int sg_plan_key_passes(const std::vector<unsigned long long> &bins, long long nPos, uint32_t seedLen, uint32_t minPasses,
+                              std::vector<uint32_t> &bounds, long long *maxN)
+{
+    size_t usable = 0, temp = 0;
+    if (sg_usable_bytes(&usable) || sg_pass_temp_bytes(nPos, nPos, seedLen, &temp)) return 1;
+    std::vector<uint64_t> bytes(SG_BUILD_BINS);
+    for (uint32_t b = 0; b < SG_BUILD_BINS; b++) bytes[b] = (uint64_t)bins[b] * 24;
+    uint32_t bad = 0;
+    if (!sg_plan_passes(bytes.data(), SG_BUILD_BINS, usable > temp ? usable - temp : 0, minPasses, bounds, &bad))
+        return sg_fail("snapgpu_index_build: the seeds whose top 16 bits are " + std::to_string(bad) + " alone need " + std::to_string(bytes[bad] + temp) +
+                       " bytes of sort scratch; " + std::to_string(usable) + " bytes of device memory are free");
+    *maxN = 0;
+    for (size_t p = 0; p + 1 < bounds.size(); p++) {
+        long long n = 0;
+        for (uint32_t b = bounds[p]; b < bounds[p + 1]; b++) n += (long long)bins[b];
+        *maxN = std::max(*maxN, n);
+    }
+    return 0;
+}
+
+// Runs fn(sortedKeys, sortedLocs, n) on the positions of each key-range pass: selected in descending location order, then
+// stable-sorted on the seed, so that equal seeds keep descending locations (as the single sweep leaves them).
+static int sg_key_pass_sweep(const uint8_t *d_bases, long long nPos, uint32_t seedLen, const std::vector<uint32_t> &bounds, long long maxN,
+                             const std::function<int(const unsigned long long *, const uint32_t *, long long)> &fn)
+{
+    SgPassScratch s;
+    size_t tempBytes = 0;
+    if (sg_pass_temp_bytes(nPos, maxN, seedLen, &tempBytes)) return 1;
+    const size_t n8 = (size_t)maxN * 8 + 16, n4 = (size_t)maxN * 4 + 16;
+    SG_CUDA(cudaMalloc((void **)&s.keys[0], n8)); SG_CUDA(cudaMalloc((void **)&s.keys[1], n8));
+    SG_CUDA(cudaMalloc((void **)&s.locs[0], n4)); SG_CUDA(cudaMalloc((void **)&s.locs[1], n4));
+    SG_CUDA(cudaMalloc(&s.temp, tempBytes)); SG_CUDA(cudaMalloc((void **)&s.nSel, 8));
+    const int grid = sg_sms() * 8;
+    for (size_t p = 0; p + 1 < bounds.size(); p++) {
+        SgBuildPassSelect pred = {d_bases, nPos, seedLen, bounds[p], bounds[p + 1]};
+        size_t tb = tempBytes;
+        SG_CUDA(cub::DeviceSelect::If(s.temp, tb, thrust::make_counting_iterator<long long>(0), s.locs[0], s.nSel, nPos, pred));
+        long long n = 0;
+        SG_CUDA(cudaMemcpy(&n, s.nSel, 8, cudaMemcpyDeviceToHost));
+        if (n > maxN) return sg_fail("snapgpu_index_build: a key-range pass selected more positions than its seeds counted");
+        if (n == 0) continue;
+        sg_build_pass_keys_kernel<<<grid, 256>>>(d_bases, nPos, seedLen, n, s.locs[0], s.keys[0]);
+        SG_CUDA(cudaGetLastError());
+        cub::DoubleBuffer<unsigned long long> kb(s.keys[0], s.keys[1]);
+        cub::DoubleBuffer<uint32_t> vb(s.locs[0], s.locs[1]);
+        tb = 0;
+        SG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, kb, vb, n, 0, (int)(2 * seedLen)));
+        if (tb > tempBytes) return sg_fail("snapgpu_index_build: sort storage larger than planned");
+        SG_CUDA(cub::DeviceRadixSort::SortPairs(s.temp, tb, kb, vb, n, 0, (int)(2 * seedLen)));
+        if (fn((const unsigned long long *)kb.Current(), (const uint32_t *)vb.Current(), n)) return 1;
+    }
+    SG_CUDA(cudaDeviceSynchronize());
+    return 0;
+}
+
 // Device-side index construction (kernels in sg_build.cuh).  d_basesPadded: SG_N_PADDING 'n', the nBases bases,
 // SG_N_PADDING 'n' -- ownership passes to the index on success.
+//
+// Memory: one sweep sorts every position at once, 24 bytes each, and keeps 12 of them while the final structures are allocated.
+// When that does not fit the free device memory (or SNAPGPU_BUILD_PASSES asks for passes), the positions are taken in key-range
+// passes (sg_build.cuh): a count sweep sizes the tables, buckets and overflow table from the exact distinct-seed counts, they are
+// allocated, and an insert sweep, planned against the memory then left, fills them.  The result is the same index either way.
 static int build_index_on_device(uint8_t *d_basesPadded, int64_t nBases, const int64_t *contigStarts, uint32_t nContigs,
                                  uint32_t seedLen, uint32_t chromosomePadding, int device, snapgpu_index **out, uint32_t layout)
 {
@@ -982,29 +1088,90 @@ static int build_index_on_device(uint8_t *d_basesPadded, int64_t nBases, const i
     void *d_temp = nullptr; size_t tempBytes = 0;
     unsigned long long *d_stats = nullptr;       // [nTables] used, then overflowWords, nValid, cursor
     int *d_failed = nullptr;
-    SG_CUDA(cudaMalloc((void **)&d_keys, (size_t)nPos * 8)); SG_CUDA(cudaMalloc((void **)&d_keys2, (size_t)nPos * 8));
-    SG_CUDA(cudaMalloc((void **)&d_locs, (size_t)nPos * 4)); SG_CUDA(cudaMalloc((void **)&d_locs2, (size_t)nPos * 4));
     const int grid = sg_sms() * 8;
-    sg_build_emit_kernel<<<grid, 256>>>(d_bases, nPos, seedLen, d_keys, d_locs);
-    SG_CUDA(cudaGetLastError());
-    cub::DoubleBuffer<unsigned long long> kb(d_keys, d_keys2);
-    cub::DoubleBuffer<uint32_t> vb(d_locs, d_locs2);
-    SG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tempBytes, kb, vb, (long long)nPos, 0, (int)(2 * seedLen + 1)));
-    SG_CUDA(cudaMalloc(&d_temp, tempBytes + 16));
-    SG_CUDA(cub::DeviceRadixSort::SortPairs(d_temp, tempBytes, kb, vb, (long long)nPos, 0, (int)(2 * seedLen + 1)));
-    SG_CUDA(cudaDeviceSynchronize());
-    cudaFree(d_temp);
-    const unsigned long long *sk = kb.Current(); const uint32_t *sv = vb.Current();
-    cudaFree(kb.Alternate()); cudaFree(vb.Alternate());
+    int hist = nTables <= 4096 ? 1 : 0;
+    if (const char *e = getenv("SNAPGPU_BUILD_SHARED_HIST")) hist = (atoi(e) != 0 && nTables <= 4096) ? 1 : 0;      // (test hook for the many-tables form)
+    auto count = [&](const unsigned long long *k, long long n) -> int {
+        sg_build_count_kernel<<<grid, 256, (size_t)((hist ? nTables : 0) + 2) * 8>>>(k, n, keyBits, seedLen, nTables, hist, d_stats, d_stats + nTables, d_stats + nTables + 1);
+        SG_CUDA(cudaGetLastError());
+        return 0;
+    };
 
-    SG_CUDA(cudaMalloc((void **)&d_stats, (size_t)(nTables + 3) * 8));
-    SG_CUDA(cudaMemset(d_stats, 0, (size_t)(nTables + 3) * 8));
-    {
-        int hist = nTables <= 4096 ? 1 : 0;
-        if (const char *e = getenv("SNAPGPU_BUILD_SHARED_HIST")) hist = (atoi(e) != 0 && nTables <= 4096) ? 1 : 0;      // (test hook for the many-tables form)
-        sg_build_count_kernel<<<grid, 256, (size_t)((hist ? nTables : 0) + 2) * 8>>>(sk, nPos, keyBits, seedLen, nTables, hist, d_stats, d_stats + nTables, d_stats + nTables + 1);
+    // One sweep when its sort (24 bytes per position) fits, and so do the 12 bytes per position it keeps beside the final structures
+    // (sized here for every position a distinct seed, at the default bucket load; the overflow table takes at most 1.5 words each).
+    const uint32_t minPasses = sg_min_passes();
+    bool onePass = minPasses == 1;
+    if (onePass) {
+        size_t usable = 0;
+        if (sg_usable_bytes(&usable)) return 1;
+        cub::DoubleBuffer<unsigned long long> kq(nullptr, nullptr);
+        cub::DoubleBuffer<uint32_t> vq(nullptr, nullptr);
+        SG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tempBytes, kq, vq, (long long)nPos, 0, (int)(2 * seedLen + 1)));
+        const double finals = layout == SG_LAYOUT_BUCKET ? (double)sg_bucket_count_for((uint64_t)nPos, seedLen, sg_bucket_default_load()) * 32
+                                                         : ((double)nPos * 1.3 + 101.0 * nTables) * 8;
+        onePass = (double)nPos * 24 + tempBytes <= (double)usable && (double)nPos * 12 + finals + (double)nPos * 6 <= (double)usable;
     }
-    SG_CUDA(cudaGetLastError());
+    std::vector<unsigned long long> bins;        // key-range passes: valid seeds per bin
+    size_t countPasses = 1;
+    const unsigned long long *sk = nullptr; const uint32_t *sv = nullptr;
+    if (onePass) {
+        SG_CUDA(cudaMalloc((void **)&d_keys, (size_t)nPos * 8)); SG_CUDA(cudaMalloc((void **)&d_keys2, (size_t)nPos * 8));
+        SG_CUDA(cudaMalloc((void **)&d_locs, (size_t)nPos * 4)); SG_CUDA(cudaMalloc((void **)&d_locs2, (size_t)nPos * 4));
+        sg_build_emit_kernel<<<grid, 256>>>(d_bases, nPos, seedLen, d_keys, d_locs);
+        SG_CUDA(cudaGetLastError());
+        cub::DoubleBuffer<unsigned long long> kb(d_keys, d_keys2);
+        cub::DoubleBuffer<uint32_t> vb(d_locs, d_locs2);
+        SG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tempBytes, kb, vb, (long long)nPos, 0, (int)(2 * seedLen + 1)));
+        SG_CUDA(cudaMalloc(&d_temp, tempBytes + 16));
+        SG_CUDA(cub::DeviceRadixSort::SortPairs(d_temp, tempBytes, kb, vb, (long long)nPos, 0, (int)(2 * seedLen + 1)));
+        SG_CUDA(cudaDeviceSynchronize());
+        cudaFree(d_temp);
+        sk = kb.Current(); sv = vb.Current();
+        cudaFree(kb.Alternate()); cudaFree(vb.Alternate());
+
+        SG_CUDA(cudaMalloc((void **)&d_stats, (size_t)(nTables + 3) * 8));
+        SG_CUDA(cudaMemset(d_stats, 0, (size_t)(nTables + 3) * 8));
+        if (count(sk, nPos)) return 1;
+    } else {
+        // count sweep: valid seeds per bin, the passes they allow, then per pass the tables' distinct seeds and overflow words
+        bins.resize(SG_BUILD_BINS);
+        unsigned long long *d_bins = nullptr;
+        SG_CUDA(cudaMalloc((void **)&d_bins, (size_t)SG_BUILD_BINS * 8));
+        SG_CUDA(cudaMemset(d_bins, 0, (size_t)SG_BUILD_BINS * 8));
+        sg_build_histogram_kernel<<<grid, 256>>>(d_bases, nPos, seedLen, d_bins);
+        SG_CUDA(cudaGetLastError());
+        SG_CUDA(cudaMemcpy(bins.data(), d_bins, (size_t)SG_BUILD_BINS * 8, cudaMemcpyDeviceToHost));
+        cudaFree(d_bins);
+        SG_CUDA(cudaMalloc((void **)&d_stats, (size_t)(nTables + 3) * 8));
+        SG_CUDA(cudaMemset(d_stats, 0, (size_t)(nTables + 3) * 8));
+        std::vector<uint32_t> bounds;
+        long long maxN = 0;
+        if (sg_plan_key_passes(bins, nPos, seedLen, minPasses, bounds, &maxN)) { cudaFree(d_stats); return 1; }
+        countPasses = bounds.size() - 1;
+        if (sg_key_pass_sweep(d_bases, nPos, seedLen, bounds, maxN, [&](const unsigned long long *k, const uint32_t *, long long n) { return count(k, n); })) {
+            cudaFree(d_stats); return 1;
+        }
+    }
+    // insert sweep: the one sorted array, or key-range passes planned against the memory left once the final structures exist
+    size_t insertPasses = 1;
+    auto insertAll = [&](unsigned long long *tables, unsigned long long *buckets, unsigned long long nB) -> int {
+        if (onePass) {
+            sg_build_insert_kernel<<<grid, 256>>>(sk, sv, nPos, keyBits, seedLen, ix->d_tableStart, ix->d_tableSize, tables, ix->d_overflow, d_stats + nTables + 2,
+                                                  nBases, d_failed, buckets, nB);
+            SG_CUDA(cudaGetLastError());
+            return 0;
+        }
+        std::vector<uint32_t> bounds;
+        long long maxN = 0;
+        if (sg_plan_key_passes(bins, nPos, seedLen, minPasses, bounds, &maxN)) return 1;
+        insertPasses = bounds.size() - 1;
+        return sg_key_pass_sweep(d_bases, nPos, seedLen, bounds, maxN, [&](const unsigned long long *k, const uint32_t *l, long long n) -> int {
+            sg_build_insert_kernel<<<grid, 256>>>(k, l, n, keyBits, seedLen, ix->d_tableStart, ix->d_tableSize, tables, ix->d_overflow, d_stats + nTables + 2,
+                                                  nBases, d_failed, buckets, nB);
+            SG_CUDA(cudaGetLastError());
+            return 0;
+        });
+    };
     std::vector<unsigned long long> stats(nTables + 3);
     SG_CUDA(cudaMemcpy(stats.data(), d_stats, (size_t)(nTables + 3) * 8, cudaMemcpyDeviceToHost));
     const unsigned long long overflowWords = stats[nTables];
@@ -1040,9 +1207,7 @@ static int build_index_on_device(uint8_t *d_basesPadded, int64_t nBases, const i
             SG_CUDA(cudaMemset(ix->d_overflow, 0, (size_t)(overflowWords + 4) * 4));
             SG_CUDA(cudaMemset(d_failed, 0, 4));
             SG_CUDA(cudaMemset(d_stats + nTables + 2, 0, 8));
-            sg_build_insert_kernel<<<grid, 256>>>(sk, sv, nPos, keyBits, seedLen, ix->d_tableStart, ix->d_tableSize, nullptr, ix->d_overflow, d_stats + nTables + 2,
-                                                  nBases, d_failed, (unsigned long long *)ix->d_buckets, nBuckets);
-            SG_CUDA(cudaGetLastError());
+            if (insertAll(nullptr, (unsigned long long *)ix->d_buckets, nBuckets)) return 1;
             int failed = 0;
             SG_CUDA(cudaMemcpy(&failed, d_failed, 4, cudaMemcpyDeviceToHost));
             done = !failed;
@@ -1056,14 +1221,15 @@ static int build_index_on_device(uint8_t *d_basesPadded, int64_t nBases, const i
         SG_CUDA(cudaGetLastError());
         SG_CUDA(cudaMemset(ix->d_overflow, 0, (size_t)(overflowWords + 4) * 4));
         SG_CUDA(cudaMemset(d_failed, 0, 4));
-        sg_build_insert_kernel<<<grid, 256>>>(sk, sv, nPos, keyBits, seedLen, ix->d_tableStart, ix->d_tableSize, (unsigned long long *)ix->d_tables,
-                                              ix->d_overflow, d_stats + nTables + 2, nBases, d_failed, nullptr, 0);
-        SG_CUDA(cudaGetLastError());
+        if (insertAll((unsigned long long *)ix->d_tables, nullptr, 0)) return 1;
         int failed = 0;
         SG_CUDA(cudaMemcpy(&failed, d_failed, 4, cudaMemcpyDeviceToHost));
         cudaFree((void *)sk); cudaFree((void *)sv); cudaFree(d_stats); cudaFree(d_failed);
         if (failed) return sg_fail("snapgpu_index_build: hash table overflow during insertion");
     }
+    if (!onePass && minPasses == 1)            // passes the free memory called for (not asked for): say so once
+        fprintf(stderr, "snapgpu_index_build: the sort did not fit the free device memory at once: %zu key-range passes to count, %zu to insert\n",
+                countPasses, insertPasses);
 
     SG_CUDA(cudaMalloc((void **)&ix->d_contigStart, (size_t)nContigs * 8 + 16));
     SG_CUDA(cudaMemcpy(ix->d_contigStart, contigStarts, (size_t)nContigs * 8, cudaMemcpyHostToDevice));
@@ -1134,22 +1300,32 @@ int snapgpu_index_save(const snapgpu_index *ix, const char *directory)
     if (ix->view.keyBytes != 4 || (ix->view.entryBytes != 8 && ix->view.entryBytes != 12))
         return sg_fail("snapgpu_index_save: unsupported entry geometry (only 4-byte keys: the image of other seed lengths is re-strided, see sg_load_index_directory)");
     SG_CUDA(cudaSetDevice(ix->device));
-    if (ix->view.layout == SG_LAYOUT_BUCKET) {
-        // The reference's directory format holds the reference's tables.  An index built on the device is built once more, in that
-        // layout, from the same bases (same hit sets, same order), written out and dropped; an index that was re-laid from a directory
-        // has that directory.
+    // The reference's directory format holds the reference's tables.  An index built on the device in sector buckets has them
+    // re-laid from its buckets (sg_build_tables_from_buckets_kernel), one range of tables at a time in a buffer that fits the free
+    // device memory, and written out in table order; its overflow table is written as it is.  An index that was re-laid from a
+    // directory has that directory.
+    const bool relay = ix->view.layout == SG_LAYOUT_BUCKET;
+    const uint32_t nT = ix->view.nTables;
+    std::vector<uint32_t> ranges = {0, nT};
+    uint64_t rangeSlots = 0;
+    struct DeviceBuffers { uint64_t *range = nullptr; int *failed = nullptr; ~DeviceBuffers() { cudaFree(range); cudaFree(failed); } } dev;
+    if (relay) {
         if (!ix->builtOnDevice) return sg_fail("snapgpu_index_save: this index was loaded from a reference-format directory (copy that), or open it with SNAPGPU_INDEX_LAYOUT=snap");
-        uint8_t *d_padded = nullptr;
-        const size_t nb = (size_t)ix->view.nBases + 2 * SG_N_PADDING;
-        SG_CUDA(cudaMalloc((void **)&d_padded, nb));
-        SG_CUDA(cudaMemcpy(d_padded, ix->d_basesPadded, nb, cudaMemcpyDeviceToDevice));
-        snapgpu_index *tmp = nullptr;
-        if (build_index_on_device(d_padded, ix->view.nBases, ix->h_contigStart.data(), (uint32_t)ix->h_contigStart.size(), ix->view.seedLen,
-                                  ix->view.chromosomePadding, ix->device, &tmp, SG_LAYOUT_SNAP)) { cudaFree(d_padded); return 1; }
-        tmp->h_contigName = ix->h_contigName; tmp->h_contigIsAlt = ix->h_contigIsAlt; tmp->h_contigOriginal = ix->h_contigOriginal;
-        const int rc = snapgpu_index_save(tmp, directory);
-        snapgpu_index_close(tmp);
-        return rc;
+        const uint32_t minPasses = sg_min_passes();
+        size_t usable = 0;
+        if (sg_usable_bytes(&usable)) return 1;
+        std::vector<uint64_t> bytes(nT);
+        for (uint32_t t = 0; t < nT; t++) bytes[t] = ix->h_tableSize[t] * 8;
+        uint32_t bad = 0;
+        if (!sg_plan_passes(bytes.data(), nT, usable > 64 ? usable - 64 : 0, minPasses, ranges, &bad))
+            return sg_fail("snapgpu_index_save: hash table " + std::to_string(bad) + " alone needs " + std::to_string(bytes[bad]) + " bytes of device memory to be re-laid; " +
+                           std::to_string(usable) + " bytes are free" + (nT == 1 ? " (seed length 16 has a single table)" : ""));
+        for (size_t p = 0; p + 1 < ranges.size(); p++)
+            rangeSlots = std::max<uint64_t>(rangeSlots, ix->h_tableStart[ranges[p + 1] - 1] + ix->h_tableSize[ranges[p + 1] - 1] - ix->h_tableStart[ranges[p]]);
+        SG_CUDA(cudaMalloc((void **)&dev.range, (size_t)rangeSlots * 8 + 16));
+        SG_CUDA(cudaMalloc((void **)&dev.failed, 4));
+        if (ranges.size() > 2 && minPasses == 1)
+            fprintf(stderr, "snapgpu_index_save: the tables did not fit the free device memory at once: %zu table-range passes\n", ranges.size() - 1);
     }
     std::string dir(directory);
     {
@@ -1201,20 +1377,36 @@ int snapgpu_index_save(const snapgpu_index *ix, const char *directory)
         FILE *f = fopen((dir + "/GenomeIndexHash").c_str(), "wb");
         if (!f) return sg_fail("snapgpu_index_save: cannot write GenomeIndexHash");
         const uint32_t eb = ix->view.entryBytes;
-        for (uint32_t t = 0; t < ix->view.nTables; t++) {
-            uint32_t magic = 0xb111b010u, ks = ix->view.keyBytes, vs = 4, vc = ix->view.large ? 2 : 1, inval = ix->view.invalidValue;
-            uint64_t tsz = ix->h_tableSize[t], used = t < ix->h_tableUsed.size() ? ix->h_tableUsed[t] : 0;
-            fwrite(&magic, 4, 1, f); fwrite(&tsz, 8, 1, f); fwrite(&used, 8, 1, f); fwrite(&ks, 4, 1, f); fwrite(&vs, 4, 1, f);
-            fwrite(&vc, 4, 1, f); fwrite(&inval, 4, 1, f);
-            hashBytes += 36;
-            size_t total = (size_t)tsz * eb;
-            const uint8_t *src = ix->view.tables + (size_t)ix->h_tableStart[t] * eb;
-            for (size_t off = 0; off < total; off += CH) {
-                size_t m = total - off < CH ? total - off : CH;
-                SG_CUDA(cudaMemcpy(buf.data(), src + off, m, cudaMemcpyDeviceToHost));
-                if (fwrite(buf.data(), 1, m, f) != m) { fclose(f); return sg_fail("snapgpu_index_save: short write"); }
+        for (size_t p = 0; p + 1 < ranges.size(); p++) {
+            const uint64_t rangeBase = ix->h_tableStart[ranges[p]];
+            if (relay) {
+                const uint64_t n = ix->h_tableStart[ranges[p + 1] - 1] + ix->h_tableSize[ranges[p + 1] - 1] - rangeBase;
+                const int grid = sg_sms() * 8;
+                sg_build_fill_kernel<<<grid, 256>>>((unsigned long long *)dev.range, (long long)n, 0x00000000ffffffffULL);
+                SG_CUDA(cudaMemset(dev.failed, 0, 4));
+                sg_build_tables_from_buckets_kernel<<<grid, 256>>>((const unsigned long long *)ix->d_buckets, ix->view.nBuckets, ix->view.seedLen, ranges[p], ranges[p + 1],
+                                                                   ix->d_tableStart, ix->d_tableSize, rangeBase, (unsigned long long *)dev.range, dev.failed);
+                SG_CUDA(cudaGetLastError());
+                int failed = 0;
+                SG_CUDA(cudaMemcpy(&failed, dev.failed, 4, cudaMemcpyDeviceToHost));
+                if (failed) { fclose(f); return sg_fail("snapgpu_index_save: a bucket slot could not be placed in the reference's tables"); }
             }
-            hashBytes += total;
+            for (uint32_t t = ranges[p]; t < ranges[p + 1]; t++) {
+                uint32_t magic = 0xb111b010u, ks = ix->view.keyBytes, vs = 4, vc = ix->view.large ? 2 : 1, inval = ix->view.invalidValue;
+                uint64_t tsz = ix->h_tableSize[t], used = t < ix->h_tableUsed.size() ? ix->h_tableUsed[t] : 0;
+                fwrite(&magic, 4, 1, f); fwrite(&tsz, 8, 1, f); fwrite(&used, 8, 1, f); fwrite(&ks, 4, 1, f); fwrite(&vs, 4, 1, f);
+                fwrite(&vc, 4, 1, f); fwrite(&inval, 4, 1, f);
+                hashBytes += 36;
+                size_t total = (size_t)tsz * eb;
+                const uint8_t *src = relay ? (const uint8_t *)dev.range + (size_t)(ix->h_tableStart[t] - rangeBase) * eb
+                                           : ix->view.tables + (size_t)ix->h_tableStart[t] * eb;
+                for (size_t off = 0; off < total; off += CH) {
+                    size_t m = total - off < CH ? total - off : CH;
+                    SG_CUDA(cudaMemcpy(buf.data(), src + off, m, cudaMemcpyDeviceToHost));
+                    if (fwrite(buf.data(), 1, m, f) != m) { fclose(f); return sg_fail("snapgpu_index_save: short write"); }
+                }
+                hashBytes += total;
+            }
         }
         fclose(f);
     }
