@@ -22,9 +22,10 @@
 extern "C" {
 #endif
 
-#define SNAPGPU_ABI_VERSION 6   /* 2: snapgpu_sam_format_* take frontClipped / clippedLens before `results`; 3: groups, replicate, host_alloc, random-sector rate;
+#define SNAPGPU_ABI_VERSION 7   /* 2: snapgpu_sam_format_* take frontClipped / clippedLens before `results`; 3: groups, replicate, host_alloc, random-sector rate;
                                  * 4: snapgpu_sam_sort_device; 5: snapgpu_bam_markdup_device, snapgpu_bam_index_device;
-                                 * 6: snapgpu_align_single_secondary(_device) (-om), snapgpu_bgzf_deflate_device, snapgpu_bam_index_members_device, snapgpu_sam_header */
+                                 * 6: snapgpu_align_single_secondary(_device) (-om), snapgpu_bgzf_deflate_device, snapgpu_bam_index_members_device, snapgpu_sam_header;
+                                 * 7: snapgpu_contig, snapgpu_index_build_genome(_device), snapgpu_save_options, snapgpu_index_save_ex */
 
 /* AlignmentResult enum, reference SNAPLib/AlignmentResult.h:34 */
 enum { SNAPGPU_NOT_FOUND = 0, SNAPGPU_SINGLE_HIT = 1, SNAPGPU_MULTIPLE_HITS = 2 };
@@ -212,10 +213,49 @@ int  snapgpu_index_build(const char *bases, int64_t nBases, const int64_t *conti
 /* Same, with the nBases bases already in HBM (DEVICE pointer); they are copied into the index image. */
 int  snapgpu_index_build_device(const char *d_bases, int64_t nBases, const int64_t *contigStarts, uint32_t nContigs,
                                 uint32_t seedLen, uint32_t chromosomePadding, int device, snapgpu_index **out);
-/* Writes the HBM-resident index out as a reference-format directory (the four files `snap-aligner index` produces,
- * SURVEY 8a-F) so stock SNAP can load an index built on the device.  A device-built bucket index has its buckets re-laid into
- * the reference's tables one range of tables at a time, in a buffer of at most the free device memory (8 bytes per table slot,
- * ~1.3 x the distinct seeds; SNAPGPU_BUILD_PASSES=n: at least n ranges).  Seed length 16 has a single table, which must fit whole. */
+/*
+ * One contig of a genome, as the reference's Genome keeps it (Genome.h Contig) and writes it to the Genome file
+ * (Genome::saveToFile): what `snap-aligner index` reads from a FASTA (names, ALT marking, ALT-last order) and an -altLiftoverFile.
+ */
+typedef struct snapgpu_contig {
+    const char *name;                   /* NUL-terminated; written with spaces as '_' */
+    int64_t  beginningLocation;         /* first base of the contig in the padded genome; ascending */
+    int32_t  isAlt;                     /* ALT contig; ALT contigs come after every non-ALT one */
+    int32_t  originalContigNumber;      /* the contig's place in the FASTA */
+    int64_t  projBeginningLocation;     /* liftover: where the ALT contig projects (the Genome file's field, as is) */
+    int32_t  projIsRC;                  /* liftover: the projection is reverse-complemented */
+    int32_t  reserved;
+    const char *projCigar;              /* liftover: the projection CIGAR; NULL without a liftover line */
+} snapgpu_contig;
+/*
+ * snapgpu_index_build(_device) with the genome's contig descriptors: the index gets their names, ALT flags, original numbers and
+ * liftover data, as snapgpu_index_open gives an index from a Genome file with ALT contigs, so it aligns ALT-aware (`snap paired`
+ * liftover) like the same genome opened from a directory `snap-aligner index` wrote.  The lookup structure is built exactly as by
+ * snapgpu_index_build.  Fails on a malformed projection CIGAR, a non-ALT contig after an ALT one, or locations that do not ascend.
+ */
+int  snapgpu_index_build_genome(const char *bases, int64_t nBases, const snapgpu_contig *contigs, uint32_t nContigs,
+                                uint32_t seedLen, uint32_t chromosomePadding, int device, snapgpu_index **out);
+int  snapgpu_index_build_genome_device(const char *d_bases, int64_t nBases, const snapgpu_contig *contigs, uint32_t nContigs,
+                                       uint32_t seedLen, uint32_t chromosomePadding, int device, snapgpu_index **out);
+/* The table geometry of a saved index: `snap-aligner index -keysize / -large / -h`. */
+typedef struct snapgpu_save_options {
+    uint32_t struct_size;               /* sizeof(snapgpu_save_options) */
+    uint32_t keyBytes;                  /* 2..8 with 2*seedLen >= 8*keyBytes and 2*seedLen - 8*keyBytes <= 16 (2..6 for seeds 16..24) */
+    uint32_t large;                     /* 1: -large tables (two values per entry, keyed by the canonical seed) */
+    uint32_t reserved;
+    double   slack;                     /* > 0: each table holds (1 + slack) x its distinct keys (at least 100 slots) */
+} snapgpu_save_options;
+/*
+ * Writes the HBM-resident index out as a reference-format directory (the four files `snap-aligner index` produces,
+ * SURVEY 8a-F) so stock SNAP can load an index built on the device.  The Genome file carries the contigs' names, ALT flags,
+ * original numbers and liftover data as given.  A device-built bucket index has its buckets re-laid into the reference's tables of
+ * the requested geometry, each table sized from its exact entry count, one range of tables at a time in buffers of at most the free
+ * device memory (a staging slot of 8 bytes -- default tables with keys of up to 4 bytes -- or 16, plus the packed entry when its
+ * size differs; SNAPGPU_BUILD_PASSES=n: at least n ranges).  A geometry with a single table needs it to fit whole.  An index in the
+ * reference's layout (SNAPGPU_INDEX_LAYOUT=snap) saves only with the default options.
+ */
+int  snapgpu_index_save_ex(const snapgpu_index *idx, const char *directory, const snapgpu_save_options *opts);
+/* snapgpu_index_save_ex with 4-byte keys, default tables and slack 0.3. */
 int  snapgpu_index_save(const snapgpu_index *idx, const char *directory);
 int  snapgpu_index_info_get(const snapgpu_index *idx, snapgpu_index_info *info);
 /*

@@ -38,6 +38,8 @@
 #include "SeedSequencer.h"
 #include "exit.h"
 #include "Error.h"
+#include "FASTA.h"
+#include "Util.h"
 
 #include <pthread.h>
 #include <string.h>
@@ -45,6 +47,8 @@
 #include <stdlib.h>
 #include <new>
 #include <vector>
+#include <string>
+#include <zlib.h>
 
 #include "../include/snapgpu.h"
 
@@ -619,7 +623,233 @@ bool GpuAlignerExtension::runIterationThread(PairedReadSupplier *supplier, Align
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------
-// snap-aligner-gpu: `single` and `paired` with the extension installed; `index` is stock.
+// `snap-aligner-gpu index-gpu <ref.fa> <dir> [options]`: `snap-aligner index` with the index built and saved on the device.  The
+// FASTA is read by the reference's own ReadFASTAGenome (names, padding, ALT marking and ordering, liftover projections); the
+// options follow `snap index`'s documented meaning.
+// ------------------------------------------------------------------------------------------------------------------------------
+static void indexGpuUsage()
+{
+    fprintf(stderr,
+        "Usage: snap-aligner-gpu index-gpu <input.fa> <output-dir> [<options>]\n"
+        "Builds a SNAP index on CUDA device 0 and writes it in the directory format of `snap-aligner index`.  Options as for\n"
+        "`snap-aligner index`:\n"
+        " -s                Seed size, 16..24 on the device (default: 24)\n"
+        " -h                Hash table slack (default: 0.3): each table holds (1 + slack) times its distinct seeds\n"
+        " -keysize          Bytes of hash table key (default: from the seed size, as `snap index`)\n"
+        " -large            Build the larger -large index (two values per entry)\n"
+        " -locationSize     Only 4 is supported; seeds below 20 need -locationSize 4 (stock defaults those to 5)\n"
+        " -p<n>             Padding between chromosomes (default: 2000)\n"
+        " -B<chars>         Chromosome name terminators in the FASTA header line\n"
+        " -bSpace / -bSpace-  Space and tab do (default) / do not end chromosome names\n"
+        " -AutoAlt-         Don't mark ALT contigs by name ('_alt' suffix, 'HLA-' prefix)\n"
+        " -maxAltContigSize Contigs at or below this size are ALT unless named otherwise below\n"
+        " -altContigName / -altContigFile        Contig names (or a file of them, one per line) to mark ALT\n"
+        " -nonAltContigName / -nonAltContigFile  Contig names (or a file of them) never to mark ALT\n"
+        " -altLiftoverFile  ALT-to-primary mappings (SAM, e.g. hs38DH.fa.alt from bwa-kit)\n"
+        " -t<n>, -sm, -exact  Accepted and without effect: the device build counts every table's seeds exactly and needs neither\n"
+        "                   host threads nor a temporary file\n"
+        " -q / -qq          Quiet: no status messages / no status or error messages\n"
+        "Not supported: -H (seed popularity histogram), location sizes other than 4.\n");
+    exit(1);
+}
+
+static void indexGpuFail(const char *what)
+{
+    WriteErrorMessage("index-gpu: %s\n", what);
+    exit(1);
+}
+
+// Lines of a (possibly gzipped) text file, without their line ends.
+static std::vector<std::string> indexGpuReadLines(const char *path, const char *what)
+{
+    std::vector<std::string> lines;
+    gzFile f = gzopen(path, "rb");
+    if (!f) { WriteErrorMessage("Unable to open %s %s\n", what, path); exit(1); }
+    std::string cur;
+    char buf[65536];
+    while (gzgets(f, buf, sizeof(buf))) {
+        cur += buf;
+        if (!cur.empty() && cur[cur.size() - 1] == '\n') {
+            while (!cur.empty() && (cur[cur.size() - 1] == '\n' || cur[cur.size() - 1] == '\r')) cur.erase(cur.size() - 1);
+            lines.push_back(cur);
+            cur.clear();
+        }
+    }
+    while (!cur.empty() && cur[cur.size() - 1] == '\r') cur.erase(cur.size() - 1);
+    if (!cur.empty()) lines.push_back(cur);
+    gzclose(f);
+    return lines;
+}
+
+// The ALT liftover file: SAM records of the ALT contigs against the primary assembly.  Per record: the ALT contig's name (QNAME),
+// the flag, the primary contig (RNAME; '*' = no projection, skipped), its 1-based position and the CIGAR.
+struct IndexGpuLiftover {
+    std::vector<std::string> names, projNames, cigars;
+    std::vector<unsigned> flags, offsets;
+};
+
+static void indexGpuReadLiftover(const char *path, IndexGpuLiftover &L)
+{
+    std::vector<std::string> lines = indexGpuReadLines(path, "ALT liftover file");
+    for (size_t i = 0; i < lines.size(); i++) {
+        const std::string &line = lines[i];
+        if (line.empty() || line[0] == '@') continue;
+        std::vector<std::string> f;
+        size_t a = 0;
+        for (;;) {
+            const size_t t = line.find('\t', a);
+            f.push_back(line.substr(a, t == std::string::npos ? std::string::npos : t - a));
+            if (t == std::string::npos) break;
+            a = t + 1;
+        }
+        unsigned flag = 0, pos = 0;
+        if (f.size() < 7 || sscanf(f[1].c_str(), "%u", &flag) != 1 || sscanf(f[3].c_str(), "%u", &pos) != 1) {
+            WriteErrorMessage("Invalid format for ALT liftover file %s. Not tab separated\n", path);
+            exit(1);
+        }
+        if (f[2].empty() || f[2][0] == '*') continue;
+        L.names.push_back(f[0]); L.flags.push_back(flag); L.projNames.push_back(f[2]); L.offsets.push_back(pos); L.cigars.push_back(f[5]);
+    }
+}
+
+static int runIndexGpu(int argc, const char **argv)
+{
+    if (argc < 2) indexGpuUsage();
+    const char *fastaFile = argv[0], *outputDir = argv[1];
+    int seedLen = 24;
+    double slack = 0.3;
+    unsigned keyBytes = 0, locationSize = 0, chromosomePadding = 2000;
+    bool large = false, spaceIsATerminator = true, autoAlt = true;
+    const char *terminators = NULL;
+    GenomeDistance maxSizeForAutomaticALT = -1;
+    std::vector<std::string> altIn, altOut;
+    IndexGpuLiftover lift;
+    for (int n = 2; n < argc; n++) {
+        const char *a = argv[n];
+        const bool hasValue = n + 1 < argc;
+        if (!strcmp(a, "-s")) { if (!hasValue) indexGpuUsage(); seedLen = atoi(argv[++n]); }
+        else if (!strcmp(a, "-h")) { if (!hasValue) indexGpuUsage(); slack = atof(argv[++n]); }
+        else if (!strcmp(a, "-exact")) {}
+        else if (!strcmp(a, "-q")) { g_suppressStatusMessages = true; }
+        else if (!strcmp(a, "-qq")) { g_suppressStatusMessages = true; g_suppressErrorMessages = true; }
+        else if (!strcmp(a, "-hg19")) { WriteErrorMessage("The -hg19 flag is deprecated, ignoring it.\n"); }
+        else if (!strcasecmp(a, "-locationSize")) {
+            if (!hasValue) indexGpuUsage();
+            locationSize = atoi(argv[++n]);
+            if (locationSize < 4 || locationSize > 8) indexGpuFail("location size must be between 4 and 8 inclusive");
+        }
+        else if (!strcmp(a, "-large")) { large = true; }
+        else if (a[0] == '-' && a[1] == 'H') { indexGpuFail("-H (seed popularity histogram) is not supported by index-gpu; use `snap-aligner index`"); }
+        else if (a[0] == '-' && a[1] == 'O') {}
+        else if (a[0] == '-' && a[1] == 't') {
+            const int t = atoi(a + 2);
+            if (t < 1 || t > 100) indexGpuFail("maxThreads must be between 1 and 100 inclusive (and you need not to leave a space after '-t')");
+        }
+        else if (a[0] == '-' && a[1] == 'p') {
+            chromosomePadding = atoi(a + 2);
+            if (chromosomePadding == 0) indexGpuFail("invalid chromosome padding specified, must be at least one");
+        }
+        else if (a[0] == '-' && a[1] == 's' && a[2] == 'm') {}
+        else if (!strcasecmp(a, "-keysize")) {
+            if (!hasValue) indexGpuUsage();
+            keyBytes = atoi(argv[++n]);
+            if (keyBytes < 2 || keyBytes > 8) indexGpuFail("key size must be between 2 and 8 inclusive");
+        }
+        else if (a[0] == '-' && a[1] == 'B') { terminators = a + 2; }
+        else if (!strcmp(a, "-bSpace")) { spaceIsATerminator = true; }
+        else if (!strcmp(a, "-bSpace-")) { spaceIsATerminator = false; }
+        else if (!strcasecmp(a, "-AutoAlt-")) { autoAlt = false; }
+        else if (!strcmp(a, "-maxAltContigSize")) { if (!hasValue) indexGpuUsage(); maxSizeForAutomaticALT = atoll(argv[++n]); }
+        else if (!strcmp(a, "-altContigName")) { if (!hasValue) indexGpuUsage(); altIn.push_back(argv[++n]); }
+        else if (!strcmp(a, "-nonAltContigName")) { if (!hasValue) indexGpuUsage(); altOut.push_back(argv[++n]); }
+        else if (!strcmp(a, "-altContigFile") || !strcmp(a, "-nonAltContigFile")) {
+            if (!hasValue) indexGpuUsage();
+            const bool in = !strcmp(a, "-altContigFile");
+            std::vector<std::string> names = indexGpuReadLines(argv[++n], in ? "alt contig list file" : "non-alt contig list file");
+            (in ? altIn : altOut).insert((in ? altIn : altOut).end(), names.begin(), names.end());
+        }
+        else if (!strcmp(a, "-altLiftoverFile")) { if (!hasValue) indexGpuUsage(); indexGpuReadLiftover(argv[++n], lift); }
+        else { WriteErrorMessage("Invalid argument: %s\n\n", a); indexGpuUsage(); }
+    }
+    if (seedLen < 16 || seedLen > 24) indexGpuFail("the device builds seeds of 16 to 24 bases; use `snap-aligner index` for other seed sizes");
+    WriteStatusMessage("Building index with seed size %d\n", seedLen);
+    if (keyBytes == 0) {
+        keyBytes = (seedLen + 2) / 4 - 1 > 2 ? (seedLen + 2) / 4 - 1 : 2;        // `snap index`'s automatic key size
+        WriteStatusMessage("Auto-set key size to %d\n", keyBytes);
+    }
+    if (locationSize == 0) {
+        locationSize = seedLen >= 20 ? 4 : 5;
+        WriteStatusMessage("Auto-set locationSize to %d\n", locationSize);
+    }
+    if (locationSize != 4) indexGpuFail("only 4-byte genome locations are supported: pass -locationSize 4 (seeds under 20 default to 5)");
+    if ((unsigned)seedLen * 2 < keyBytes * 8) indexGpuFail("you must specify a smaller keysize or a larger seed size: the seed must fill the key");
+    if (seedLen * 2 - (int)keyBytes * 8 > 16) indexGpuFail("you must specify a bigger keysize or smaller seed size: at most 4^8 hash tables");
+    if (!(slack > 0)) indexGpuFail("the hash table slack must be positive");
+    WriteStatusMessage("Hash table slack %lf\nLoading FASTA file '%s' into memory...", slack, fastaFile);
+
+    _int64 start = timeInMillis();
+    std::vector<const char *> inNames, outNames;
+    for (size_t i = 0; i < altIn.size(); i++) inNames.push_back(altIn[i].c_str());
+    for (size_t i = 0; i < altOut.size(); i++) outNames.push_back(altOut[i].c_str());
+    std::vector<char *> lNames, lProj, lCigar;
+    for (size_t i = 0; i < lift.names.size(); i++) {
+        lNames.push_back((char *)lift.names[i].c_str()); lProj.push_back((char *)lift.projNames[i].c_str()); lCigar.push_back((char *)lift.cigars[i].c_str());
+    }
+    const int nLift = (int)lift.names.size();
+    const Genome *genome = ReadFASTAGenome(fastaFile, terminators, spaceIsATerminator, chromosomePadding, inNames.empty() ? NULL : &inNames[0], (int)inNames.size(),
+                                           outNames.empty() ? NULL : &outNames[0], (int)outNames.size(), maxSizeForAutomaticALT, autoAlt,
+                                           nLift ? &lNames[0] : NULL, nLift ? &lift.flags[0] : NULL, nLift ? &lProj[0] : NULL, nLift ? &lift.offsets[0] : NULL,
+                                           nLift ? &lCigar[0] : NULL, nLift);
+    if (genome == NULL) indexGpuFail("unable to read FASTA file");
+    const _int64 readMs = timeInMillis() - start;
+    WriteStatusMessage("%llds\n", (readMs + 500) / 1000);
+    char b1[40], b2[40];
+    WriteStatusMessage("Genome has %s contigs, of which %s are ALTs\n", FormatUIntWithCommas(genome->getNumContigs(), b1, sizeof(b1)),
+                       FormatUIntWithCommas(genome->getNumALTContigs(), b2, sizeof(b2)));
+    const GenomeDistance nBases = genome->getCountOfBases();
+    if (nBases > ((_int64)1 << 32) - 16) indexGpuFail("genome is too big for 4-byte genome locations, the only size the device index supports");
+
+    std::vector<snapgpu_contig> contigs(genome->getNumContigs());
+    for (int i = 0; i < genome->getNumContigs(); i++) {
+        const Genome::Contig *c = genome->getContigByInternalNumber(InternalContigNum(i));
+        snapgpu_contig &d = contigs[i];
+        memset(&d, 0, sizeof(d));
+        d.name = c->name;
+        d.beginningLocation = GenomeLocationAsInt64(c->beginningLocation);
+        d.isAlt = c->isALT ? 1 : 0;
+        d.originalContigNumber = OriginalContigNumToInt(c->originalContigNumber);
+        d.projBeginningLocation = GenomeLocationAsInt64(c->projBeginningLocation);
+        d.projIsRC = c->isProjRC ? 1 : 0;
+        d.projCigar = c->projCigar;
+    }
+    WriteStatusMessage("Building the index on the device...");
+    start = timeInMillis();
+    snapgpu_index *ix = NULL;
+    if (snapgpu_index_build_genome(genome->getSubstring(0, 0), nBases, &contigs[0], (uint32_t)contigs.size(), (uint32_t)seedLen, chromosomePadding, 0, &ix)) {
+        WriteErrorMessage("index-gpu: %s\n", snapgpu_last_error());
+        exit(1);
+    }
+    const _int64 buildMs = timeInMillis() - start;
+    snapgpu_index_info info;
+    snapgpu_index_info_get(ix, &info);
+    WriteStatusMessage("%.2fs (%lld HBM bytes)\nSaving index to '%s'...", buildMs / 1000.0, (long long)info.hbmBytes, outputDir);
+    start = timeInMillis();
+    snapgpu_save_options o;
+    memset(&o, 0, sizeof(o));
+    o.struct_size = sizeof(o); o.keyBytes = keyBytes; o.large = large ? 1 : 0; o.slack = slack;
+    if (snapgpu_index_save_ex(ix, outputDir, &o)) {
+        WriteErrorMessage("index-gpu: %s\n", snapgpu_last_error());
+        exit(1);
+    }
+    const _int64 saveMs = timeInMillis() - start;
+    snapgpu_index_close(ix);
+    WriteStatusMessage("%.2fs\nIndex build and save took %.2fs (FASTA read %.2fs, device build %.2fs, save %.2fs)\n", saveMs / 1000.0,
+                       (readMs + buildMs + saveMs) / 1000.0, readMs / 1000.0, buildMs / 1000.0, saveMs / 1000.0);
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------------------------------------
+// snap-aligner-gpu: `single` and `paired` with the extension installed; `index` is stock, `index-gpu` builds on the device.
 // ------------------------------------------------------------------------------------------------------------------------------
 #ifndef SNAPGPU_EXTENSION_NO_MAIN
 static const char *GPU_VERSION = "2.0.5-snapgpu";
@@ -627,7 +857,7 @@ static const char *GPU_VERSION = "2.0.5-snapgpu";
 int main(int argc, const char **argv)
 {
     if (argc < 2) {
-        fprintf(stderr, "Usage: snap-aligner-gpu <index|single|paired> [<options>]   (options as for snap-aligner)\n");
+        fprintf(stderr, "Usage: snap-aligner-gpu <index|index-gpu|single|paired> [<options>]   (options as for snap-aligner)\n");
         return 1;
     }
     InitializeSeedSequencers();
@@ -635,6 +865,7 @@ int main(int argc, const char **argv)
         GenomeIndex::runIndexer(argc - 2, argv + 2);
         return 0;
     }
+    if (strcmp(argv[1], "index-gpu") == 0) return runIndexGpu(argc - 2, argv + 2);
     for (int i = 1; i < argc; ) {
         unsigned nArgsConsumed = 0;
         if (strcmp(argv[i], "single") == 0) {

@@ -124,6 +124,127 @@ SG_HD bool sg_bucket_slot_decode(uint64_t slot, uint64_t b, uint64_t nBuckets, u
     return false;
 }
 
+// ---- re-laying buckets into the reference's tables of any geometry (snapgpu_index_save_ex on the device, sg_host.h on the host) ----
+// A table entry is keyBytes bytes of key after 1 value (default tables) or 2 (-large) of 4 bytes.  The table of a key is its seed's
+// bits above the low 8 * keyBytes; default tables key the seed as it lies in the genome, -large tables the smaller of the seed and
+// its reverse complement, with value 0 for the locations of that canonical seed and value 1 for those of its reverse complement
+// (GenomeIndex.cpp:1528-1570).  A seed that is its own reverse complement fills value 0 only, as it has only orientation 0 here.
+//
+// Entries are 6..14 bytes in the file, so they are first inserted into an aligned staging form, slot for slot:
+//   8 bytes  (default tables, keyBytes <= 4): key << 32 | value, empty = value 0xffffffff and key 0, as in the reference;
+//   16 bytes (-large, or keyBytes > 4):       u64 key + 1 (0: empty), then the two values, 0xfffffffe where unused,
+// and then packed to the file stride (sg_relay_pack).
+SG_HD uint64_t sg_fmix64(uint64_t key);                                             // sg_seed.h
+SG_HD uint64_t sg_table_probe_next(uint64_t idx, uint64_t nProbes, uint64_t size); // sg_seed.h
+
+#define SG_RELAY_EMPTY8 0x00000000ffffffffULL
+
+SG_HD uint32_t sg_relay_stage_bytes(uint32_t keyBytes, uint32_t large) { return (!large && keyBytes <= 4) ? 8u : 16u; }
+SG_HD uint32_t sg_relay_file_bytes(uint32_t keyBytes, uint32_t large) { return (large ? 8u : 4u) + keyBytes; }
+
+// Geometries the reference's `snap index` accepts for a seed length (GenomeIndex.cpp runIndexer): the seed fills the key, and at most
+// 4^8 tables.
+SG_HD bool sg_relay_geometry_ok(uint32_t seedLen, uint32_t keyBytes)
+{
+    return keyBytes >= 2 && keyBytes <= 8 && 2 * seedLen >= 8 * keyBytes && 2 * seedLen - 8 * keyBytes <= 16;
+}
+
+// The entry a used slot of bucket b becomes: its table, key and which value it fills.  False if the slot does not decode.
+SG_HD bool sg_relay_entry(uint64_t slot, uint64_t b, uint64_t nBuckets, uint32_t seedLen, uint32_t keyBytes, uint32_t large,
+                          uint32_t *table, uint64_t *key, uint32_t *which)
+{
+    uint64_t seed; uint32_t orient;
+    if (!sg_bucket_slot_decode(slot, b, nBuckets, seedLen, &seed, &orient)) return false;
+    const uint64_t k = (large && orient) ? sg_seed_revcomp(seed, seedLen) : seed;     // -large: back to the canonical seed
+    const uint32_t keyBits = 8 * keyBytes;
+    *table = (uint32_t)(k >> keyBits);
+    *key = keyBits >= 64 ? k : (k & ((1ULL << keyBits) - 1));
+    *which = large ? orient : 0u;
+    return true;
+}
+
+// Whether the buckets hold (canonical, orient): a -large entry is counted once, by its orientation-0 slot when there is one.
+SG_HD bool sg_bucket_holds(const uint64_t *buckets, uint64_t nBuckets, uint32_t bits, uint64_t canonical, uint32_t orient)
+{
+    const uint64_t h = sg_bucket_mix(canonical, bits);
+    uint64_t b = sg_bucket_home(h, bits, nBuckets);
+    const uint64_t want = ((uint64_t)orient << 62) | ((h & 0x3fffffffULL) << 32);
+    for (int disp = 0; disp <= SG_BUCKET_MAX_DISP; disp++) {
+        for (int k = 0; k < SG_BUCKET_SLOTS; k++) {
+            const uint64_t s = buckets[b * SG_BUCKET_SLOTS + k];
+            if ((s & 0x7fffffff00000000ULL) == want && (uint32_t)s != 0xffffffffu) return true;
+        }
+        if (!(buckets[b * SG_BUCKET_SLOTS] & SG_BUCKET_FLAG)) return false;
+        b = (b + 1 == nBuckets) ? 0 : b + 1;
+    }
+    return false;
+}
+
+// Whether a used slot of bucket b counts as an entry of its table (which it gets) in the given geometry.
+SG_HD bool sg_relay_counts(const uint64_t *buckets, uint64_t nBuckets, uint64_t s, uint32_t seedLen, uint32_t keyBytes, uint32_t large, uint32_t *table, bool *ok)
+{
+    const uint64_t slot = buckets[s];
+    *ok = true;
+    if ((uint32_t)slot == 0xffffffffu) return false;
+    uint64_t key; uint32_t which;
+    if (!sg_relay_entry(slot, s / SG_BUCKET_SLOTS, nBuckets, seedLen, keyBytes, large, table, &key, &which)) { *ok = false; return false; }
+    // SNAPHashTable::Insert counts an entry when it changes the slot's key (HashTable.cpp:329-332), and an empty slot's key is 0: the
+    // reference's used count leaves out key 0, and so does the count written here
+    if (key == 0) return false;
+    if (which == 1) {
+        const uint64_t canonical = ((uint64_t)*table << (8 * keyBytes)) | key;
+        if (sg_bucket_holds(buckets, nBuckets, 2 * seedLen, canonical, 0)) return false;
+    }
+    return true;
+}
+
+// Sequential insertion into one table's staging slots (stage: the table's first slot), along SNAPHashTable's probe sequence;
+// the device does the same with compare-and-swap (sg_build.cuh).  False if the table is full.
+SG_HD bool sg_relay_insert_seq(uint8_t *stage, uint32_t stageBytes, uint64_t size, uint64_t key, uint32_t which, uint32_t value)
+{
+    uint64_t idx = sg_fmix64(key) % size;
+    for (uint64_t nProbes = 0;;) {
+        uint64_t *p = (uint64_t *)(stage + idx * stageBytes);
+        if (stageBytes == 8) {
+            if (p[0] == SG_RELAY_EMPTY8) { p[0] = (key << 32) | value; return true; }
+        } else if (p[0] == 0 || p[0] == key + 1) {
+            p[0] = key + 1;
+            ((uint32_t *)(p + 1))[which] = value;
+            return true;
+        }
+        if (++nProbes > size + 5) return false;
+        idx = sg_table_probe_next(idx, nProbes, size);
+    }
+}
+
+// The staging slots' initial content
+SG_HD void sg_relay_stage_clear(uint8_t *slot, uint32_t stageBytes)
+{
+    uint64_t *p = (uint64_t *)slot;
+    if (stageBytes == 8) { p[0] = SG_RELAY_EMPTY8; return; }
+    p[0] = 0;
+    p[1] = 0xfffffffefffffffeULL;
+}
+
+// Staging slot i -> file entry i (values, then the key's keyBytes bytes, little-endian); an empty slot becomes the reference's
+// empty entry (value 0 invalid, key 0).
+SG_HD void sg_relay_pack(const uint8_t *stage, uint32_t stageBytes, uint64_t i, uint8_t *out, uint32_t keyBytes, uint32_t large)
+{
+    const uint64_t *p = (const uint64_t *)(stage + i * stageBytes);
+    uint32_t v[2] = {0xffffffffu, 0u};
+    uint64_t key = 0;
+    if (stageBytes == 8) {
+        v[0] = (uint32_t)p[0]; key = p[0] >> 32;
+    } else if (p[0] != 0) {
+        key = p[0] - 1; v[0] = (uint32_t)p[1]; v[1] = (uint32_t)(p[1] >> 32);
+    }
+    uint8_t *e = out + i * sg_relay_file_bytes(keyBytes, large);
+    const uint32_t nv = large ? 2u : 1u;
+    for (uint32_t j = 0; j < nv; j++)
+        for (uint32_t k = 0; k < 4; k++) e[4 * j + k] = (uint8_t)(v[j] >> (8 * k));
+    for (uint32_t k = 0; k < keyBytes; k++) e[4 * nv + k] = (uint8_t)(key >> (8 * k));
+}
+
 // The four slots of bucket b, one sector.
 struct SgBucket { uint64_t s[SG_BUCKET_SLOTS]; };
 

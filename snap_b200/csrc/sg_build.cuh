@@ -262,23 +262,76 @@ __global__ void sg_build_pass_keys_kernel(const uint8_t *bases, long long nPosit
     }
 }
 
-// ---- saving a bucket index in the reference's layout (snapgpu_index_save), one range of tables per pass ----
-// Every used bucket slot becomes the entry (seed, value) of its table, its value unchanged (a location, or countOfBases + an
-// offset into the index's own overflow table).  tables: the range's tables back to back, table t at tableStart[t] - rangeBase.
-__global__ void sg_build_tables_from_buckets_kernel(const unsigned long long *buckets, unsigned long long nBuckets, uint32_t seedLen,
-                                                    uint32_t tableLo, uint32_t tableHi, const uint64_t *tableStart, const uint64_t *tableSize,
-                                                    uint64_t rangeBase, unsigned long long *tables, int *failed)
+// ---- saving a bucket index in the reference's layout, any key size, default or -large tables (snapgpu_index_save_ex) ----
+// Every used bucket slot becomes (a value of) an entry of its table, its value unchanged (a location, or countOfBases + an offset
+// into the index's own overflow table); sg_bucket.h has the mapping, the staging form and the packing.
+
+// Entries per table in the target geometry.  Few tables: a per-block shared histogram, added to the global one once per block.
+#define SG_RELAY_SHARED_TABLES 8192u
+__global__ void sg_relay_count_kernel(const unsigned long long *buckets, unsigned long long nBuckets, uint32_t seedLen, uint32_t keyBytes, uint32_t large,
+                                      uint32_t nTables, unsigned long long *used, int *failed)
+{
+    __shared__ uint32_t sUsed[SG_RELAY_SHARED_TABLES];
+    const bool shared = nTables <= SG_RELAY_SHARED_TABLES;
+    if (shared) for (uint32_t t = threadIdx.x; t < nTables; t += blockDim.x) sUsed[t] = 0;
+    __syncthreads();
+    const unsigned long long nSlots = nBuckets * SG_BUCKET_SLOTS;
+    for (unsigned long long s = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; s < nSlots; s += (unsigned long long)gridDim.x * blockDim.x) {
+        uint32_t t; bool ok;
+        if (sg_relay_counts((const uint64_t *)buckets, nBuckets, s, seedLen, keyBytes, large, &t, &ok)) {
+            if (shared) atomicAdd(&sUsed[t], 1u); else atomicAdd(&used[t], 1ULL);
+        }
+        if (!ok) *failed = 1;
+    }
+    __syncthreads();
+    if (shared) for (uint32_t t = threadIdx.x; t < nTables; t += blockDim.x) if (sUsed[t]) atomicAdd(&used[t], (unsigned long long)sUsed[t]);
+}
+
+// sg_relay_insert_seq with compare-and-swap: an 8-byte slot is claimed whole; a 16-byte slot is claimed (or found) by its key word,
+// and the value this slot fills is then its own word (the two orientations of a -large entry come from two bucket slots).
+__device__ __forceinline__ bool sg_relay_insert_atomic(uint8_t *stage, uint32_t stageBytes, uint64_t size, unsigned long long key, uint32_t which, uint32_t value)
+{
+    uint64_t idx = sg_fmix64(key) % size;
+    for (unsigned long long nProbes = 0;;) {
+        unsigned long long *p = (unsigned long long *)(stage + idx * stageBytes);
+        if (stageBytes == 8) {
+            if (atomicCAS(p, SG_RELAY_EMPTY8, (key << 32) | value) == SG_RELAY_EMPTY8) return true;
+        } else {
+            const unsigned long long prev = atomicCAS(p, 0ULL, key + 1);
+            if (prev == 0 || prev == key + 1) { ((uint32_t *)(p + 1))[which] = value; return true; }
+        }
+        if (++nProbes > size + 5) return false;
+        idx = sg_table_probe_next(idx, nProbes, size);
+    }
+}
+
+// The entries of tables [tableLo, tableHi) into their staging slots: table t at slot tableStart[t] - rangeBase of `stage`.
+__global__ void sg_relay_insert_kernel(const unsigned long long *buckets, unsigned long long nBuckets, uint32_t seedLen, uint32_t keyBytes, uint32_t large,
+                                       uint32_t tableLo, uint32_t tableHi, const uint64_t *tableStart, const uint64_t *tableSize, uint64_t rangeBase,
+                                       uint8_t *stage, uint32_t stageBytes, int *failed)
 {
     const unsigned long long nSlots = nBuckets * SG_BUCKET_SLOTS;
     for (unsigned long long s = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; s < nSlots; s += (unsigned long long)gridDim.x * blockDim.x) {
         const unsigned long long slot = buckets[s];
         if ((uint32_t)slot == 0xffffffffu) continue;
-        uint64_t seed; uint32_t orient;
-        if (!sg_bucket_slot_decode(slot, s / SG_BUCKET_SLOTS, nBuckets, seedLen, &seed, &orient)) { *failed = 1; continue; }
-        const uint32_t t = (uint32_t)(seed >> 32);
+        uint32_t t, which; uint64_t key;
+        if (!sg_relay_entry(slot, s / SG_BUCKET_SLOTS, nBuckets, seedLen, keyBytes, large, &t, &key, &which)) { *failed = 1; continue; }
         if (t < tableLo || t >= tableHi) continue;
-        if (!sg_table_insert_atomic(tables + (tableStart[t] - rangeBase), tableSize[t], seed & 0xffffffffULL, (uint32_t)slot)) *failed = 1;
+        if (!sg_relay_insert_atomic(stage + (size_t)(tableStart[t] - rangeBase) * stageBytes, stageBytes, tableSize[t], key, which, (uint32_t)slot)) *failed = 1;
     }
+}
+
+__global__ void sg_relay_stage_clear_kernel(uint8_t *stage, uint32_t stageBytes, unsigned long long n)
+{
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x)
+        sg_relay_stage_clear(stage + i * stageBytes, stageBytes);
+}
+
+// staging slots [0, n) -> file entries at their stride (6..14 bytes), back to back
+__global__ void sg_relay_pack_kernel(const uint8_t *stage, uint32_t stageBytes, unsigned long long n, uint8_t *out, uint32_t keyBytes, uint32_t large)
+{
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x)
+        sg_relay_pack(stage, stageBytes, i, out, keyBytes, large);
 }
 
 __global__ void sg_build_fill_kernel(unsigned long long *p, long long n, unsigned long long v)

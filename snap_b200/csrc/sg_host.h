@@ -12,6 +12,15 @@
 #include "sg_common.h"
 #include "sg_seed.h"
 
+// One contig line of the Genome file (Genome::saveToFile, Genome.cpp:216-228), field for field: beginningLocation, the ALT flag,
+// originalContigNumber, the projection start and its reverse-complement flag, the name, the projection CIGAR ("*" for none).
+struct SgContigLine {
+    int64_t start = 0, projStart = 0;
+    uint32_t flags = 0, projFlags = 0;
+    int32_t original = 0;
+    std::string name, projCigar = "*";
+};
+
 struct SgHostIndex {
     std::vector<uint8_t>  tables;        // repacked: entries of all tables back to back (+8 bytes slack)
     std::vector<uint64_t> tableStart, tableSize, tableUsed, tableMagic;
@@ -21,6 +30,7 @@ struct SgHostIndex {
     std::vector<uint8_t>  contigIsAlt;
     std::vector<int32_t>  contigOriginal;   // Genome::Contig::originalContigNumber (order in the FASTA; what sorted output is ordered by)
     std::vector<std::string> contigName;
+    std::vector<SgContigLine> contigLines;   // the Genome file's contig lines as read (sg_set_contigs)
     // ALT liftover data of each contig line (SgIndexView::projStart / projRC / projOps); empty when no contig is ALT
     std::vector<int64_t>  projStart;
     std::vector<uint8_t>  projRC;
@@ -48,6 +58,97 @@ struct SgHostIndex {
         return v;
     }
 };
+
+// The contig metadata of an index from its Genome file lines, as Genome::loadFromFile keeps it (Genome.cpp:348-403): starts, names,
+// ALT flags, original numbers, and the liftover arrays when some contig is ALT.  False on a malformed projection CIGAR, or an ALT
+// contig followed by a non-ALT one (the index keeps the ALTs last, FASTA.cpp, so genomeLocationOfFirstALTContig bounds them).
+static inline bool sg_set_contigs(SgHostIndex &ix, const std::vector<SgContigLine> &lines, std::string &err)
+{
+    ix.contigLines = lines;
+    ix.contigStart.clear(); ix.contigIsAlt.clear(); ix.contigName.clear(); ix.contigOriginal.clear();
+    ix.projStart.clear(); ix.projRC.clear(); ix.projOps.clear();
+    std::vector<uint32_t> projOpBegin, ops;
+    for (size_t i = 0; i < lines.size(); i++) {
+        const SgContigLine &L = lines[i];
+        if (i > 0 && ix.contigIsAlt.back() && !(L.flags & 1)) { err = "Genome contigs: a non-ALT contig follows an ALT contig (ALT contigs must come last)"; return false; }
+        ix.contigStart.push_back(L.start);
+        ix.contigIsAlt.push_back((L.flags & 1) ? 1 : 0);
+        ix.contigOriginal.push_back(L.original);
+        ix.contigName.push_back(L.name);
+        ix.projStart.push_back(L.projStart);
+        ix.projRC.push_back(0);
+        projOpBegin.push_back((uint32_t)ops.size());
+        // a CIGAR of length 1 is the "*" of a contig without a liftover line (Genome.cpp:380-401)
+        if (L.projCigar.size() > 1) {
+            const char *c = L.projCigar.data(), *ce = c + L.projCigar.size();
+            while (c < ce) {
+                long long count = 0; const char *d = c;
+                while (c < ce && *c >= '0' && *c <= '9') { count = count * 10 + (*c - '0'); c++; if (count > 0x7fffffLL) break; }
+                if (c == d || c >= ce || count > 0x7fffffLL || !*c || !strchr("MIDNSHP=X", *c)) { err = "Genome contig line: malformed projection CIGAR"; return false; }
+                ops.push_back(((uint32_t)count << 8) | (uint8_t)*c);
+                c++;
+            }
+            ix.projRC.back() = (L.projFlags & 1) ? 1 : 0;       // GENOME_FLAG_ALT_PROJ_CONTIG_IS_RC
+        }
+    }
+    projOpBegin.push_back((uint32_t)ops.size());
+    if (std::find(ix.contigIsAlt.begin(), ix.contigIsAlt.end(), (uint8_t)1) == ix.contigIsAlt.end()) {
+        ix.projStart.clear(); ix.projRC.clear();        // nothing can be lifted over
+    } else {
+        for (size_t c = 0; c < projOpBegin.size(); c++) ix.projOps.push_back((uint32_t)projOpBegin.size() + projOpBegin[c]);
+        ix.projOps.insert(ix.projOps.end(), ops.begin(), ops.end());
+    }
+    // genomeLocationOfFirstALTContig, Genome.cpp:460-476
+    ix.altFirstLocation = LLONG_MAX;
+    for (size_t i = 0; i < ix.contigStart.size(); i++)
+        if (ix.contigIsAlt[i] && ix.contigStart[i] < ix.altFirstLocation) ix.altFirstLocation = ix.contigStart[i];
+    return true;
+}
+
+// The text of a Genome file before its bases (Genome::saveToFile): the header line, then one line per contig, a name's spaces
+// written as '_' as the reference does (the line is space-separated).
+static inline std::string sg_genome_file_header(int64_t nBases, const std::vector<SgContigLine> &lines)
+{
+    std::string out;
+    char buf[160];
+    snprintf(buf, sizeof(buf), "%lld %d %d\n", (long long)nBases, (int)lines.size(), 1);       // GENOME_FLAG_ALT_CONTIGS_MARKED
+    out += buf;
+    for (size_t c = 0; c < lines.size(); c++) {
+        const SgContigLine &L = lines[c];
+        std::string name = L.name;
+        for (size_t k = 0; k < name.size(); k++) if (name[k] == ' ') name[k] = '_';
+        snprintf(buf, sizeof(buf), "%lld %x %d %lld %x %d %d ", (long long)L.start, L.flags, (int)L.original, (long long)L.projStart, L.projFlags,
+                 (int)name.size(), (int)L.projCigar.size());
+        out += buf; out += name; out += ' '; out += L.projCigar; out += '\n';
+    }
+    return out;
+}
+
+// The GenomeIndex file (GenomeIndex.cpp:1007-1008): major minor nHashTables overflowTableSize seedLen chromosomePadding keySize
+// hashTablesFileSize smallHashTable locationSize
+static inline std::string sg_genome_index_text(uint32_t nTables, uint64_t overflowSize, uint32_t seedLen, uint32_t chromosomePadding, uint32_t keyBytes,
+                                               uint64_t hashBytes, uint32_t large)
+{
+    char buf[200];
+    snprintf(buf, sizeof(buf), "%d %d %d %lld %d %d %d %lld %d %d", 7, 1, (int)nTables, (long long)overflowSize, (int)seedLen, (int)chromosomePadding,
+             (int)keyBytes, (long long)hashBytes, large ? 0 : 1, 4);
+    return buf;
+}
+
+// A table's header in GenomeIndexHash (SNAPHashTable::saveToFile, HashTable.cpp:199-240): 36 bytes
+static inline void sg_table_header(uint8_t out[36], uint64_t size, uint64_t used, uint32_t keyBytes, uint32_t large, uint32_t invalidValue)
+{
+    const uint32_t magic = 0xb111b010u, vs = 4, vc = large ? 2 : 1;
+    memcpy(out, &magic, 4); memcpy(out + 4, &size, 8); memcpy(out + 12, &used, 8); memcpy(out + 20, &keyBytes, 4);
+    memcpy(out + 24, &vs, 4); memcpy(out + 28, &vc, 4); memcpy(out + 32, &invalidValue, 4);
+}
+
+// Slots of a table holding `used` entries: (1 + slack) x its content (GenomeIndex.cpp:1084-1100 with exact counts), at least 100
+static inline uint64_t sg_table_slots(uint64_t used, double slack)
+{
+    const uint64_t sz = (uint64_t)((double)used * (1.0 + slack)) + 1;
+    return sz < 100 ? 100 : sz;
+}
 
 static inline bool sg_read_file(const std::string &path, std::vector<uint8_t> &out, std::string &err)
 {
@@ -93,9 +194,7 @@ static inline bool sg_load_index_directory(const std::string &dir, SgHostIndex &
         if (!nl || 3 != sscanf(p, "%lld %d %d", &nBases, &nContigs, &flags)) { err = "Genome header unparsable"; return false; }
         p = nl + 1;
         ix.nBases = nBases;
-        ix.contigStart.clear(); ix.contigIsAlt.clear(); ix.contigName.clear(); ix.contigOriginal.clear();
-        ix.projStart.clear(); ix.projRC.clear();
-        std::vector<uint32_t> projOpBegin, ops;
+        std::vector<SgContigLine> lines;
         for (int i = 0; i < nContigs; i++) {
             nl = (const char *)memchr(p, '\n', endp - p);
             if (!nl) { err = "Genome contig line truncated"; return false; }
@@ -106,45 +205,21 @@ static inline bool sg_load_index_directory(const std::string &dir, SgHostIndex &
             // name starts after the 7th space
             const char *q = p; int spaces = 0;
             while (q < nl && spaces < 7) { if (*q == ' ') spaces++; q++; }
-            ix.contigStart.push_back(start);
-            ix.contigIsAlt.push_back((cflags & 1) ? 1 : 0);
-            ix.contigOriginal.push_back(origNum);
             if (nameLen < 0 || (long long)nameLen > (long long)(nl - q)) { err = "Genome contig line: name length runs past the line"; return false; }
-            ix.contigName.push_back(std::string(q, (size_t)nameLen));
-            // the projection CIGAR follows the name; a length of 1 is the "*" of a contig without a liftover line (Genome.cpp:380-401)
-            ix.projStart.push_back(projStart);
-            ix.projRC.push_back(0);
-            projOpBegin.push_back((uint32_t)ops.size());
-            if (cigarLen > 1) {
-                const char *c = q + nameLen + 1;
-                if (c + cigarLen > nl) { err = "Genome contig line: projection CIGAR runs past the line"; return false; }
-                const char *ce = c + cigarLen;
-                while (c < ce) {
-                    long long count = 0; const char *d = c;
-                    while (c < ce && *c >= '0' && *c <= '9') { count = count * 10 + (*c - '0'); c++; if (count > 0x7fffffLL) break; }
-                    if (c == d || c >= ce || count > 0x7fffffLL || !strchr("MIDNSHP=X", *c)) { err = "Genome contig line: malformed projection CIGAR"; return false; }
-                    ops.push_back(((uint32_t)count << 8) | (uint8_t)*c);
-                    c++;
-                }
-                ix.projRC.back() = (projRC & 1) ? 1 : 0;       // GENOME_FLAG_ALT_PROJ_CONTIG_IS_RC
-            }
+            SgContigLine L;
+            L.start = start; L.flags = cflags; L.original = origNum; L.projStart = projStart; L.projFlags = projRC;
+            L.name.assign(q, (size_t)nameLen);
+            // the projection CIGAR follows the name ("*" without a liftover line)
+            const char *c = q + nameLen + 1;
+            if (cigarLen < 0 || c > nl || (long long)cigarLen > (long long)(nl - c)) { err = "Genome contig line: projection CIGAR runs past the line"; return false; }
+            L.projCigar.assign(c, (size_t)cigarLen);
+            lines.push_back(L);
             p = nl + 1;
         }
-        projOpBegin.push_back((uint32_t)ops.size());
-        ix.projOps.clear();
-        if (std::find(ix.contigIsAlt.begin(), ix.contigIsAlt.end(), (uint8_t)1) == ix.contigIsAlt.end()) {
-            ix.projStart.clear(); ix.projRC.clear();        // nothing can be lifted over
-        } else {
-            for (size_t c = 0; c < projOpBegin.size(); c++) ix.projOps.push_back((uint32_t)projOpBegin.size() + projOpBegin[c]);
-            ix.projOps.insert(ix.projOps.end(), ops.begin(), ops.end());
-        }
+        if (!sg_set_contigs(ix, lines, err)) return false;
         if ((long long)(endp - p) != nBases) { err = "Genome: base count does not match file size"; return false; }
         ix.basesPadded.assign((size_t)nBases + 2 * SG_N_PADDING, (uint8_t)'n');
         memcpy(ix.basesPadded.data() + SG_N_PADDING, p, (size_t)nBases);
-        // genomeLocationOfFirstALTContig, Genome.cpp:460-476
-        ix.altFirstLocation = LLONG_MAX;
-        for (size_t i = 0; i < ix.contigStart.size(); i++)
-            if (ix.contigIsAlt[i] && ix.contigStart[i] < ix.altFirstLocation) ix.altFirstLocation = ix.contigStart[i];
     }
 
     // --- OverflowTable: raw u32[]
@@ -266,34 +341,53 @@ static inline bool sg_host_relayout(SgHostIndex &ix, double load, std::string &e
     return false;
 }
 
-// Writes the reference's tables (tableStart / tableSize / invalidValue as they stand) from the sector buckets: every used slot
-// becomes one (seed, value) entry, placed along SNAPHashTable's probe sequence.  The sequential form of what snapgpu_index_save
-// does on the device for an index built there; the host-side tests use it.  Recomputes tableUsed; afterwards view() hands out
-// the tables.
-static inline bool sg_host_buckets_to_tables(SgHostIndex &ix, std::string &err)
+// Entries per table of the bucket-layout index re-laid into the reference's tables of the given geometry (sg_bucket.h): the
+// sequential form of sg_relay_count_kernel.
+static inline bool sg_host_relay_count(const SgHostIndex &ix, uint32_t keyBytes, uint32_t large, std::vector<uint64_t> &used, std::string &err)
 {
-    if (ix.layout != SG_LAYOUT_BUCKET || ix.large || ix.entryBytes != 8 || ix.keyBytes != 4) { err = "buckets -> tables needs a bucket-layout index with 8-byte entries"; return false; }
-    const uint32_t keyBits = 32;
-    const uint64_t empty = (uint64_t)ix.invalidValue;                    // key 0, value invalid
-    std::vector<uint64_t> t64((size_t)ix.totalSlots + 2, empty);
-    ix.tableUsed.assign(ix.nTables, 0);
+    if (ix.layout != SG_LAYOUT_BUCKET || !sg_relay_geometry_ok(ix.seedLen, keyBytes)) { err = "re-lay needs a bucket-layout index and a key size the seed fills"; return false; }
+    used.assign((size_t)1 << (2 * ix.seedLen - 8 * keyBytes), 0);
+    for (uint64_t s = 0; s < ix.nBuckets * SG_BUCKET_SLOTS; s++) {
+        uint32_t t; bool ok;
+        if (sg_relay_counts(ix.buckets.data(), ix.nBuckets, s, ix.seedLen, keyBytes, large, &t, &ok)) used[t]++;
+        if (!ok) { err = "a bucket slot is out of reach of its home"; return false; }
+    }
+    return true;
+}
+
+// Re-lays the buckets into the reference's tables of the given geometry, table t with tableSize[t] slots: `packed` gets the tables
+// back to back at the file's entry stride.  The sequential form of what snapgpu_index_save_ex does on the device, through the same
+// staging form and probe sequence.
+static inline bool sg_host_relay_tables(const SgHostIndex &ix, uint32_t keyBytes, uint32_t large, const std::vector<uint64_t> &tableSize,
+                                        std::vector<uint8_t> &packed, std::string &err)
+{
+    const uint32_t sb = sg_relay_stage_bytes(keyBytes, large), fb = sg_relay_file_bytes(keyBytes, large);
+    std::vector<uint64_t> start(tableSize.size() + 1, 0);
+    for (size_t t = 0; t < tableSize.size(); t++) start[t + 1] = start[t] + tableSize[t];
+    std::vector<uint8_t> stage((size_t)start.back() * sb);
+    for (uint64_t i = 0; i < start.back(); i++) sg_relay_stage_clear(stage.data() + i * sb, sb);
     for (uint64_t s = 0; s < ix.nBuckets * SG_BUCKET_SLOTS; s++) {
         const uint64_t slot = ix.buckets[s];
         if ((uint32_t)slot == 0xffffffffu) continue;
-        uint64_t seed; uint32_t orient;
-        if (!sg_bucket_slot_decode(slot, s / SG_BUCKET_SLOTS, ix.nBuckets, ix.seedLen, &seed, &orient)) { err = "a bucket slot is out of reach of its home"; return false; }
-        const uint32_t t = (uint32_t)(seed >> keyBits);
-        const uint64_t low = seed & 0xffffffffULL, size = ix.tableSize[t], base = ix.tableStart[t];
-        uint64_t idx = sg_fmix64(low) % size, nProbes = 0;
-        while (t64[base + idx] != empty) {
-            if (++nProbes > size + 5) { err = "hash table overflow"; return false; }
-            idx = sg_table_probe_next(idx, nProbes, size);
-        }
-        t64[base + idx] = (low << 32) | (uint32_t)slot;
-        ix.tableUsed[t]++;
+        uint32_t t, which; uint64_t key;
+        if (!sg_relay_entry(slot, s / SG_BUCKET_SLOTS, ix.nBuckets, ix.seedLen, keyBytes, large, &t, &key, &which)) { err = "a bucket slot is out of reach of its home"; return false; }
+        if (t >= tableSize.size()) { err = "re-lay: table out of range"; return false; }
+        if (!sg_relay_insert_seq(stage.data() + (size_t)start[t] * sb, sb, tableSize[t], key, which, (uint32_t)slot)) { err = "hash table overflow"; return false; }
     }
-    ix.tables.assign((size_t)ix.totalSlots * 8 + 16, 0);
-    memcpy(ix.tables.data(), t64.data(), (size_t)ix.totalSlots * 8);
+    packed.assign((size_t)start.back() * fb, 0);
+    for (uint64_t i = 0; i < start.back(); i++) sg_relay_pack(stage.data(), sb, i, packed.data(), keyBytes, large);
+    return true;
+}
+
+// Writes the reference's tables (tableStart / tableSize as they stand, the index's own key size and table kind) from the sector
+// buckets, recounting tableUsed; afterwards view() hands out the tables.  The host-side tests use it.
+static inline bool sg_host_buckets_to_tables(SgHostIndex &ix, std::string &err)
+{
+    if (ix.layout != SG_LAYOUT_BUCKET || ix.keyBytes != 4) { err = "buckets -> tables needs a bucket-layout index with 4-byte keys"; return false; }
+    std::vector<uint8_t> packed;
+    if (!sg_host_relay_count(ix, ix.keyBytes, ix.large, ix.tableUsed, err) || !sg_host_relay_tables(ix, ix.keyBytes, ix.large, ix.tableSize, packed, err)) return false;
+    packed.resize(packed.size() + 16, 0);
+    ix.tables.swap(packed);
     ix.layout = SG_LAYOUT_SNAP;
     ix.buckets.clear(); ix.nBuckets = 0;
     return true;

@@ -85,6 +85,7 @@ struct snapgpu_index {
     std::vector<int64_t> h_projStart;
     std::vector<uint8_t> h_projRC;
     std::vector<uint32_t> h_projOps;
+    std::vector<SgContigLine> h_contigLines; // the Genome file's contig lines (written back by snapgpu_index_save_ex)
 };
 
 struct snapgpu_aligner {
@@ -943,6 +944,7 @@ static int upload_index(const SgHostIndex &h, int device, snapgpu_index **out)
     ix->info.overflowTableSize = h.overflowSize; ix->info.hashTableSlots = h.totalSlots; ix->info.hbmBytes = hbm;
     ix->h_tableStart = h.tableStart; ix->h_tableSize = h.tableSize; ix->h_tableUsed = h.tableUsed;
     ix->h_contigStart = h.contigStart; ix->h_contigName = h.contigName; ix->h_contigIsAlt = h.contigIsAlt; ix->h_contigOriginal = h.contigOriginal;
+    ix->h_contigLines = h.contigLines;
     ix->view.layout = SG_LAYOUT_SNAP; ix->view.pad0 = 0; ix->view.buckets = nullptr; ix->view.nBuckets = 0;
     if (wanted_layout() == SG_LAYOUT_BUCKET) {
         if (relayout_on_device(ix, &hbm)) { snapgpu_index_close(ix); return 1; }
@@ -1070,11 +1072,19 @@ static int sg_key_pass_sweep(const uint8_t *d_bases, long long nPos, uint32_t se
 // When that does not fit the free device memory (or SNAPGPU_BUILD_PASSES asks for passes), the positions are taken in key-range
 // passes (sg_build.cuh): a count sweep sizes the tables, buckets and overflow table from the exact distinct-seed counts, they are
 // allocated, and an insert sweep, planned against the memory then left, fills them.  The result is the same index either way.
-static int build_index_on_device(uint8_t *d_basesPadded, int64_t nBases, const int64_t *contigStarts, uint32_t nContigs,
+// `contigs`: the Genome file's contig lines; the index keeps their names, ALT flags and liftover data as snapgpu_index_open does.
+static int build_index_on_device(uint8_t *d_basesPadded, int64_t nBases, const std::vector<SgContigLine> &contigs,
                                  uint32_t seedLen, uint32_t chromosomePadding, int device, snapgpu_index **out, uint32_t layout)
 {
     if (seedLen < 16 || seedLen > 24) return sg_fail("snapgpu_index_build: seed length must be in [16, 24]");
     if (nBases <= (int64_t)seedLen + 2 || nBases > 0xffffffffLL - 16) return sg_fail("snapgpu_index_build: genome size unsupported for 4-byte locations");
+    SgHostIndex meta;
+    std::string metaErr;
+    if (!sg_set_contigs(meta, contigs, metaErr)) return sg_fail("snapgpu_index_build: " + metaErr);
+    for (size_t c = 0; c < contigs.size(); c++)
+        if (contigs[c].start < 0 || contigs[c].start >= nBases || (c > 0 && contigs[c].start <= contigs[c - 1].start))
+            return sg_fail("snapgpu_index_build: contig beginning locations must ascend within the genome");
+    const uint32_t nContigs = (uint32_t)contigs.size();
     const uint32_t keyBytes = 4, keyBits = 32;
     const uint32_t nTables = 1u << ((seedLen - 16) * 2);
     const long long nPos = nBases - seedLen - 1;          // GenomeIndex.cpp:645-652: locations [0, countOfBases - seedLen - 1)
@@ -1181,8 +1191,7 @@ static int build_index_on_device(uint8_t *d_basesPadded, int64_t nBases, const i
     std::vector<uint64_t> tstart(nTables), tsize(nTables), tmagic(nTables);
     uint64_t slots = 0, distinct = 0;
     for (uint32_t t = 0; t < nTables; t++) {
-        uint64_t sz = (uint64_t)((double)stats[t] * 1.3) + 1;
-        if (sz < 100) sz = 100;
+        const uint64_t sz = sg_table_slots(stats[t], 0.3);
         tstart[t] = slots; tsize[t] = sz; tmagic[t] = ~0ULL / sz; slots += sz;
         distinct += stats[t];
     }
@@ -1232,7 +1241,16 @@ static int build_index_on_device(uint8_t *d_basesPadded, int64_t nBases, const i
                 countPasses, insertPasses);
 
     SG_CUDA(cudaMalloc((void **)&ix->d_contigStart, (size_t)nContigs * 8 + 16));
-    SG_CUDA(cudaMemcpy(ix->d_contigStart, contigStarts, (size_t)nContigs * 8, cudaMemcpyHostToDevice));
+    SG_CUDA(cudaMemcpy(ix->d_contigStart, meta.contigStart.data(), (size_t)nContigs * 8, cudaMemcpyHostToDevice));
+    if (!meta.projStart.empty()) {             // ALT liftover arrays, as upload_index places them
+        SG_CUDA(cudaMalloc((void **)&ix->d_projStart, meta.projStart.size() * 8));
+        SG_CUDA(cudaMemcpy(ix->d_projStart, meta.projStart.data(), meta.projStart.size() * 8, cudaMemcpyHostToDevice));
+        SG_CUDA(cudaMalloc((void **)&ix->d_projRC, meta.projRC.size() + 16));
+        SG_CUDA(cudaMemcpy(ix->d_projRC, meta.projRC.data(), meta.projRC.size(), cudaMemcpyHostToDevice));
+        SG_CUDA(cudaMalloc((void **)&ix->d_projOps, meta.projOps.size() * 4));
+        SG_CUDA(cudaMemcpy(ix->d_projOps, meta.projOps.data(), meta.projOps.size() * 4, cudaMemcpyHostToDevice));
+        hbm += meta.projStart.size() * 8 + meta.projRC.size() + 16 + meta.projOps.size() * 4;
+    }
     sg_init_tables(ix->h_tables_prob, seedLen);
     SG_CUDA(cudaMalloc((void **)&ix->d_tables_prob, sizeof(SgTables)));
     SG_CUDA(cudaMemcpy(ix->d_tables_prob, &ix->h_tables_prob, sizeof(SgTables), cudaMemcpyHostToDevice));
@@ -1241,7 +1259,8 @@ static int build_index_on_device(uint8_t *d_basesPadded, int64_t nBases, const i
     SgIndexView v;
     memset(&v, 0, sizeof(v));
     v.tables = ix->d_tables; v.tableStart = ix->d_tableStart; v.tableSize = ix->d_tableSize; v.tableMagic = ix->d_tableMagic; v.overflow = ix->d_overflow;
-    v.bases = d_bases; v.contigStart = ix->d_contigStart; v.nBases = nBases; v.altFirstLocation = LLONG_MAX;
+    v.bases = d_bases; v.contigStart = ix->d_contigStart; v.nBases = nBases; v.altFirstLocation = meta.altFirstLocation;
+    v.projStart = ix->d_projStart; v.projRC = ix->d_projRC; v.projOps = ix->d_projOps;
     v.overflowSize = overflowWords; v.nContigs = nContigs; v.seedLen = seedLen; v.keyBytes = keyBytes; v.nTables = nTables;
     v.large = 0; v.entryBytes = 8; v.chromosomePadding = chromosomePadding; v.invalidValue = 0xffffffffu;
     v.layout = layout; v.pad0 = 0; v.buckets = ix->d_buckets; v.nBuckets = nBuckets;
@@ -1254,10 +1273,53 @@ static int build_index_on_device(uint8_t *d_basesPadded, int64_t nBases, const i
     ix->info.reserved = layout;
     ix->h_tableStart = tstart; ix->h_tableSize = tsize;
     ix->h_tableUsed.assign(stats.begin(), stats.begin() + nTables);
-    ix->h_contigStart.assign(contigStarts, contigStarts + nContigs);
-    for (uint32_t c = 0; c < nContigs; c++) { ix->h_contigName.push_back("chr" + std::to_string(c + 1)); ix->h_contigIsAlt.push_back(0); ix->h_contigOriginal.push_back((int32_t)c); }
+    ix->h_contigStart = meta.contigStart; ix->h_contigName = meta.contigName; ix->h_contigIsAlt = meta.contigIsAlt; ix->h_contigOriginal = meta.contigOriginal;
+    ix->h_projStart = meta.projStart; ix->h_projRC = meta.projRC; ix->h_projOps = meta.projOps;
+    ix->h_contigLines = contigs;
     *out = ix;
     return 0;
+}
+
+// The contig lines an index built from bases and contig starts alone gets: contigs chr1..chrN, none ALT, no liftover.
+static std::vector<SgContigLine> plain_contigs(const int64_t *contigStarts, uint32_t nContigs)
+{
+    std::vector<SgContigLine> lines(nContigs);
+    for (uint32_t c = 0; c < nContigs; c++) { lines[c].start = contigStarts[c]; lines[c].original = (int32_t)c; lines[c].name = "chr" + std::to_string(c + 1); }
+    return lines;
+}
+
+// snapgpu_contig descriptors -> the Genome file's contig lines, checked: names present, beginning locations ascending inside the genome
+static int described_contigs(const snapgpu_contig *contigs, uint32_t nContigs, int64_t nBases, std::vector<SgContigLine> &lines)
+{
+    lines.assign(nContigs, SgContigLine());
+    for (uint32_t c = 0; c < nContigs; c++) {
+        const snapgpu_contig &d = contigs[c];
+        if (!d.name) return sg_fail("snapgpu_index_build_genome: contig " + std::to_string(c) + " has no name");
+        if (d.beginningLocation < 0 || d.beginningLocation >= nBases || (c > 0 && d.beginningLocation <= contigs[c - 1].beginningLocation))
+            return sg_fail("snapgpu_index_build_genome: contig beginning locations must ascend within the genome (contig " + std::to_string(c) + ")");
+        SgContigLine &L = lines[c];
+        L.start = d.beginningLocation; L.flags = d.isAlt ? 1u : 0u; L.original = d.originalContigNumber;
+        L.projStart = d.projBeginningLocation; L.projFlags = d.projIsRC ? 1u : 0u;
+        L.name = d.name;
+        L.projCigar = d.projCigar ? d.projCigar : "*";
+    }
+    return 0;
+}
+
+// Copies the nBases bases (host or device memory) between SG_N_PADDING 'n' on each side, then builds; the padded copy passes to
+// the index.
+static int build_from(const char *bases, bool onDevice, int64_t nBases, const std::vector<SgContigLine> &contigs, uint32_t seedLen,
+                      uint32_t chromosomePadding, int device, snapgpu_index **out)
+{
+    if (require_device(device)) return 1;
+    if (nBases <= 0) return sg_fail("snapgpu_index_build: empty genome");
+    uint8_t *d_padded = nullptr;
+    SG_CUDA(cudaMalloc((void **)&d_padded, (size_t)nBases + 2 * SG_N_PADDING));
+    SG_CUDA(cudaMemset(d_padded, 'n', (size_t)nBases + 2 * SG_N_PADDING));
+    SG_CUDA(cudaMemcpy(d_padded + SG_N_PADDING, bases, (size_t)nBases, onDevice ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+    int rc = build_index_on_device(d_padded, nBases, contigs, seedLen, chromosomePadding, device, out, wanted_layout());
+    if (rc) cudaFree(d_padded);
+    return rc;
 }
 
 int snapgpu_index_build(const char *bases, int64_t nBases, const int64_t *contigStarts, uint32_t nContigs,
@@ -1265,14 +1327,7 @@ int snapgpu_index_build(const char *bases, int64_t nBases, const int64_t *contig
 {
     if (!bases || !contigStarts || !out || nContigs == 0) return sg_fail("null argument");
     *out = nullptr;
-    if (require_device(device)) return 1;
-    uint8_t *d_padded = nullptr;
-    SG_CUDA(cudaMalloc((void **)&d_padded, (size_t)nBases + 2 * SG_N_PADDING));
-    SG_CUDA(cudaMemset(d_padded, 'n', (size_t)nBases + 2 * SG_N_PADDING));
-    SG_CUDA(cudaMemcpy(d_padded + SG_N_PADDING, bases, (size_t)nBases, cudaMemcpyHostToDevice));
-    int rc = build_index_on_device(d_padded, nBases, contigStarts, nContigs, seedLen, chromosomePadding, device, out, wanted_layout());
-    if (rc) cudaFree(d_padded);
-    return rc;
+    return build_from(bases, false, nBases, plain_contigs(contigStarts, nContigs), seedLen, chromosomePadding, device, out);
 }
 
 // Same, from bases already in HBM (d_bases: nBases bytes, device pointer); copies them into the index image.
@@ -1281,51 +1336,103 @@ int snapgpu_index_build_device(const char *d_bases, int64_t nBases, const int64_
 {
     if (!d_bases || !contigStarts || !out || nContigs == 0) return sg_fail("null argument");
     *out = nullptr;
-    if (require_device(device)) return 1;
-    uint8_t *d_padded = nullptr;
-    SG_CUDA(cudaMalloc((void **)&d_padded, (size_t)nBases + 2 * SG_N_PADDING));
-    SG_CUDA(cudaMemset(d_padded, 'n', (size_t)nBases + 2 * SG_N_PADDING));
-    SG_CUDA(cudaMemcpy(d_padded + SG_N_PADDING, d_bases, (size_t)nBases, cudaMemcpyDeviceToDevice));
-    int rc = build_index_on_device(d_padded, nBases, contigStarts, nContigs, seedLen, chromosomePadding, device, out, wanted_layout());
-    if (rc) cudaFree(d_padded);
-    return rc;
+    return build_from(d_bases, true, nBases, plain_contigs(contigStarts, nContigs), seedLen, chromosomePadding, device, out);
+}
+
+int snapgpu_index_build_genome(const char *bases, int64_t nBases, const snapgpu_contig *contigs, uint32_t nContigs,
+                               uint32_t seedLen, uint32_t chromosomePadding, int device, snapgpu_index **out)
+{
+    if (!bases || !contigs || !out || nContigs == 0) return sg_fail("null argument");
+    *out = nullptr;
+    std::vector<SgContigLine> lines;
+    if (described_contigs(contigs, nContigs, nBases, lines)) return 1;
+    return build_from(bases, false, nBases, lines, seedLen, chromosomePadding, device, out);
+}
+
+int snapgpu_index_build_genome_device(const char *d_bases, int64_t nBases, const snapgpu_contig *contigs, uint32_t nContigs,
+                                      uint32_t seedLen, uint32_t chromosomePadding, int device, snapgpu_index **out)
+{
+    if (!d_bases || !contigs || !out || nContigs == 0) return sg_fail("null argument");
+    *out = nullptr;
+    std::vector<SgContigLine> lines;
+    if (described_contigs(contigs, nContigs, nBases, lines)) return 1;
+    return build_from(d_bases, true, nBases, lines, seedLen, chromosomePadding, device, out);
 }
 
 // Writes the index out in the reference's own 4-file directory format (v7.1: GenomeIndex.cpp:1007-1008 header,
 // HashTable.cpp:199-260 table headers, GenomeIndex.cpp:964-988 overflow, Genome.cpp:203-253 genome), so that the
-// stock `snap-aligner` can load an index built by snapgpu_index_build.
-int snapgpu_index_save(const snapgpu_index *ix, const char *directory)
+// stock `snap-aligner` can load an index built by snapgpu_index_build, in the table geometry `o` asks for.
+int snapgpu_index_save_ex(const snapgpu_index *ix, const char *directory, const snapgpu_save_options *o)
 {
-    if (!ix || !directory) return sg_fail("null argument");
-    if (ix->view.keyBytes != 4 || (ix->view.entryBytes != 8 && ix->view.entryBytes != 12))
-        return sg_fail("snapgpu_index_save: unsupported entry geometry (only 4-byte keys: the image of other seed lengths is re-strided, see sg_load_index_directory)");
+    if (!ix || !directory || !o) return sg_fail("null argument");
+    if (o->struct_size != sizeof(snapgpu_save_options)) return sg_fail("snapgpu_save_options.struct_size mismatch (ABI)");
+    const uint32_t seedLen = ix->view.seedLen, kb = o->keyBytes, large = o->large ? 1u : 0u;
+    const double slack = o->slack;
+    const bool relay = ix->view.layout == SG_LAYOUT_BUCKET;
+    if ((relay || !(kb == 4 && !large && slack == 0.3)) && !sg_relay_geometry_ok(seedLen, kb))
+        return sg_fail("snapgpu_index_save_ex: a " + std::to_string(kb) + "-byte key does not suit seed length " + std::to_string(seedLen) +
+                       " (the seed must fill the key and leave at most 16 bits of table number: 2*seedLen >= 8*keyBytes and 2*seedLen - 8*keyBytes <= 16)");
+    if (!(slack > 0.0 && slack <= 100.0)) return sg_fail("snapgpu_index_save_ex: slack must be positive (the reference's default is 0.3)");
+    const bool defaults = kb == 4 && !large && slack == 0.3;
     SG_CUDA(cudaSetDevice(ix->device));
     // The reference's directory format holds the reference's tables.  An index built on the device in sector buckets has them
-    // re-laid from its buckets (sg_build_tables_from_buckets_kernel), one range of tables at a time in a buffer that fits the free
-    // device memory, and written out in table order; its overflow table is written as it is.  An index that was re-laid from a
-    // directory has that directory.
-    const bool relay = ix->view.layout == SG_LAYOUT_BUCKET;
-    const uint32_t nT = ix->view.nTables;
+    // re-laid from its buckets in the requested geometry: entries per table counted (sg_relay_count_kernel) and tables sized from
+    // the counts, then one range of tables at a time, in staging buffers that fit the free device memory, inserted
+    // (sg_relay_insert_kernel), packed to the file's entry stride and written out in table order; its overflow table is written as it
+    // is.  An index in the reference's layout writes its own tables.
+    uint32_t nT = ix->view.nTables, keyBytes = ix->view.keyBytes, isLarge = ix->view.large;
+    std::vector<uint64_t> tstart = ix->h_tableStart, tsize = ix->h_tableSize, tused = ix->h_tableUsed;
     std::vector<uint32_t> ranges = {0, nT};
     uint64_t rangeSlots = 0;
-    struct DeviceBuffers { uint64_t *range = nullptr; int *failed = nullptr; ~DeviceBuffers() { cudaFree(range); cudaFree(failed); } } dev;
+    uint32_t stageBytes = 0, fileBytes = 0;
+    struct DeviceBuffers {
+        uint8_t *stage = nullptr, *packed = nullptr; uint64_t *tableStart = nullptr, *tableSize = nullptr; unsigned long long *used = nullptr; int *failed = nullptr;
+        ~DeviceBuffers() { cudaFree(stage); cudaFree(packed); cudaFree(tableStart); cudaFree(tableSize); cudaFree(used); cudaFree(failed); }
+    } dev;
     if (relay) {
         if (!ix->builtOnDevice) return sg_fail("snapgpu_index_save: this index was loaded from a reference-format directory (copy that), or open it with SNAPGPU_INDEX_LAYOUT=snap");
+        nT = 1u << (2 * seedLen - 8 * kb); keyBytes = kb; isLarge = large;
+        stageBytes = sg_relay_stage_bytes(kb, large); fileBytes = sg_relay_file_bytes(kb, large);
+        const int grid = sg_sms() * 8;
+        SG_CUDA(cudaMalloc((void **)&dev.used, (size_t)nT * 8)); SG_CUDA(cudaMemset(dev.used, 0, (size_t)nT * 8));
+        SG_CUDA(cudaMalloc((void **)&dev.failed, 4)); SG_CUDA(cudaMemset(dev.failed, 0, 4));
+        sg_relay_count_kernel<<<grid, 256>>>((const unsigned long long *)ix->d_buckets, ix->view.nBuckets, seedLen, kb, large, nT, dev.used, dev.failed);
+        SG_CUDA(cudaGetLastError());
+        tused.assign(nT, 0);
+        int failed = 0;
+        SG_CUDA(cudaMemcpy(tused.data(), dev.used, (size_t)nT * 8, cudaMemcpyDeviceToHost));
+        SG_CUDA(cudaMemcpy(&failed, dev.failed, 4, cudaMemcpyDeviceToHost));
+        if (failed) return sg_fail("snapgpu_index_save: a bucket slot is out of reach of its home bucket");
+        tstart.assign(nT, 0); tsize.assign(nT, 0);
+        uint64_t slots = 0;
+        for (uint32_t t = 0; t < nT; t++) { tsize[t] = sg_table_slots(tused[t], slack); tstart[t] = slots; slots += tsize[t]; }
+        SG_CUDA(cudaMalloc((void **)&dev.tableStart, (size_t)nT * 8)); SG_CUDA(cudaMalloc((void **)&dev.tableSize, (size_t)nT * 8));
+        SG_CUDA(cudaMemcpy(dev.tableStart, tstart.data(), (size_t)nT * 8, cudaMemcpyHostToDevice));
+        SG_CUDA(cudaMemcpy(dev.tableSize, tsize.data(), (size_t)nT * 8, cudaMemcpyHostToDevice));
+        // a range's device bytes per slot: the staging form, and the packed entries when their stride differs from it
+        const uint32_t perSlot = stageBytes + (fileBytes != stageBytes ? fileBytes : 0);
         const uint32_t minPasses = sg_min_passes();
         size_t usable = 0;
         if (sg_usable_bytes(&usable)) return 1;
         std::vector<uint64_t> bytes(nT);
-        for (uint32_t t = 0; t < nT; t++) bytes[t] = ix->h_tableSize[t] * 8;
+        for (uint32_t t = 0; t < nT; t++) bytes[t] = tsize[t] * perSlot;
         uint32_t bad = 0;
         if (!sg_plan_passes(bytes.data(), nT, usable > 64 ? usable - 64 : 0, minPasses, ranges, &bad))
             return sg_fail("snapgpu_index_save: hash table " + std::to_string(bad) + " alone needs " + std::to_string(bytes[bad]) + " bytes of device memory to be re-laid; " +
-                           std::to_string(usable) + " bytes are free" + (nT == 1 ? " (seed length 16 has a single table)" : ""));
+                           std::to_string(usable) + " bytes are free" + (nT == 1 ? " (this geometry has a single table)" : ""));
         for (size_t p = 0; p + 1 < ranges.size(); p++)
-            rangeSlots = std::max<uint64_t>(rangeSlots, ix->h_tableStart[ranges[p + 1] - 1] + ix->h_tableSize[ranges[p + 1] - 1] - ix->h_tableStart[ranges[p]]);
-        SG_CUDA(cudaMalloc((void **)&dev.range, (size_t)rangeSlots * 8 + 16));
-        SG_CUDA(cudaMalloc((void **)&dev.failed, 4));
+            rangeSlots = std::max<uint64_t>(rangeSlots, tstart[ranges[p + 1] - 1] + tsize[ranges[p + 1] - 1] - tstart[ranges[p]]);
+        SG_CUDA(cudaMalloc((void **)&dev.stage, (size_t)rangeSlots * stageBytes + 16));
+        if (fileBytes != stageBytes) SG_CUDA(cudaMalloc((void **)&dev.packed, (size_t)rangeSlots * fileBytes + 16));
         if (ranges.size() > 2 && minPasses == 1)
             fprintf(stderr, "snapgpu_index_save: the tables did not fit the free device memory at once: %zu table-range passes\n", ranges.size() - 1);
+    } else {
+        if (!defaults)
+            return sg_fail(std::string("snapgpu_index_save_ex: an index in the reference's table layout (") +
+                           (ix->builtOnDevice ? "built on the device with SNAPGPU_INDEX_LAYOUT=snap" : "opened from a directory") +
+                           ") saves only with the default options: 4-byte keys, default tables, slack 0.3");
+        if (ix->view.keyBytes != 4 || (ix->view.entryBytes != 8 && ix->view.entryBytes != 12))
+            return sg_fail("snapgpu_index_save: unsupported entry geometry (only 4-byte keys: the image of other seed lengths is re-strided, see sg_load_index_directory)");
     }
     std::string dir(directory);
     {
@@ -1345,13 +1452,8 @@ int snapgpu_index_save(const snapgpu_index *ix, const char *directory)
     {
         FILE *f = fopen((dir + "/Genome").c_str(), "wb");
         if (!f) return sg_fail("snapgpu_index_save: cannot write Genome");
-        fprintf(f, "%lld %d %d\n", (long long)ix->view.nBases, (int)ix->h_contigStart.size(), 1);
-        for (size_t c = 0; c < ix->h_contigStart.size(); c++) {
-            std::string name = ix->h_contigName[c];
-            for (size_t k = 0; k < name.size(); k++) if (name[k] == ' ') name[k] = '_';      // Genome::saveToFile does the same (Genome.cpp:230-236): the line is space-separated
-            fprintf(f, "%lld %x %d %lld %x %d %d %s %s\n", (long long)ix->h_contigStart[c], ix->h_contigIsAlt[c] ? 1 : 0, (int)ix->h_contigOriginal[c], 0LL, 0,
-                    (int)name.size(), 1, name.c_str(), "*");
-        }
+        const std::string head = sg_genome_file_header(ix->view.nBases, ix->h_contigLines);
+        if (fwrite(head.data(), 1, head.size(), f) != head.size()) { fclose(f); return sg_fail("snapgpu_index_save: short write"); }
         for (size_t off = 0; off < (size_t)ix->view.nBases; off += CH) {
             size_t m = (size_t)ix->view.nBases - off < CH ? (size_t)ix->view.nBases - off : CH;
             SG_CUDA(cudaMemcpy(buf.data(), ix->view.bases + off, m, cudaMemcpyDeviceToHost));
@@ -1376,30 +1478,35 @@ int snapgpu_index_save(const snapgpu_index *ix, const char *directory)
     {
         FILE *f = fopen((dir + "/GenomeIndexHash").c_str(), "wb");
         if (!f) return sg_fail("snapgpu_index_save: cannot write GenomeIndexHash");
-        const uint32_t eb = ix->view.entryBytes;
+        const uint32_t eb = relay ? fileBytes : ix->view.entryBytes;
         for (size_t p = 0; p + 1 < ranges.size(); p++) {
-            const uint64_t rangeBase = ix->h_tableStart[ranges[p]];
+            const uint64_t rangeBase = tstart[ranges[p]];
+            const uint8_t *out = nullptr;
             if (relay) {
-                const uint64_t n = ix->h_tableStart[ranges[p + 1] - 1] + ix->h_tableSize[ranges[p + 1] - 1] - rangeBase;
+                const uint64_t n = tstart[ranges[p + 1] - 1] + tsize[ranges[p + 1] - 1] - rangeBase;
                 const int grid = sg_sms() * 8;
-                sg_build_fill_kernel<<<grid, 256>>>((unsigned long long *)dev.range, (long long)n, 0x00000000ffffffffULL);
+                sg_relay_stage_clear_kernel<<<grid, 256>>>(dev.stage, stageBytes, n);
                 SG_CUDA(cudaMemset(dev.failed, 0, 4));
-                sg_build_tables_from_buckets_kernel<<<grid, 256>>>((const unsigned long long *)ix->d_buckets, ix->view.nBuckets, ix->view.seedLen, ranges[p], ranges[p + 1],
-                                                                   ix->d_tableStart, ix->d_tableSize, rangeBase, (unsigned long long *)dev.range, dev.failed);
+                sg_relay_insert_kernel<<<grid, 256>>>((const unsigned long long *)ix->d_buckets, ix->view.nBuckets, seedLen, kb, large, ranges[p], ranges[p + 1],
+                                                      dev.tableStart, dev.tableSize, rangeBase, dev.stage, stageBytes, dev.failed);
                 SG_CUDA(cudaGetLastError());
                 int failed = 0;
                 SG_CUDA(cudaMemcpy(&failed, dev.failed, 4, cudaMemcpyDeviceToHost));
                 if (failed) { fclose(f); return sg_fail("snapgpu_index_save: a bucket slot could not be placed in the reference's tables"); }
+                out = dev.stage;
+                if (dev.packed) {
+                    sg_relay_pack_kernel<<<grid, 256>>>(dev.stage, stageBytes, n, dev.packed, kb, large);
+                    SG_CUDA(cudaGetLastError());
+                    out = dev.packed;
+                }
             }
             for (uint32_t t = ranges[p]; t < ranges[p + 1]; t++) {
-                uint32_t magic = 0xb111b010u, ks = ix->view.keyBytes, vs = 4, vc = ix->view.large ? 2 : 1, inval = ix->view.invalidValue;
-                uint64_t tsz = ix->h_tableSize[t], used = t < ix->h_tableUsed.size() ? ix->h_tableUsed[t] : 0;
-                fwrite(&magic, 4, 1, f); fwrite(&tsz, 8, 1, f); fwrite(&used, 8, 1, f); fwrite(&ks, 4, 1, f); fwrite(&vs, 4, 1, f);
-                fwrite(&vc, 4, 1, f); fwrite(&inval, 4, 1, f);
+                uint8_t head[36];
+                sg_table_header(head, tsize[t], t < tused.size() ? tused[t] : 0, keyBytes, isLarge, ix->view.invalidValue);
+                if (fwrite(head, 1, 36, f) != 36) { fclose(f); return sg_fail("snapgpu_index_save: short write"); }
                 hashBytes += 36;
-                size_t total = (size_t)tsz * eb;
-                const uint8_t *src = relay ? (const uint8_t *)dev.range + (size_t)(ix->h_tableStart[t] - rangeBase) * eb
-                                           : ix->view.tables + (size_t)ix->h_tableStart[t] * eb;
+                size_t total = (size_t)tsize[t] * eb;
+                const uint8_t *src = relay ? out + (size_t)(tstart[t] - rangeBase) * eb : ix->view.tables + (size_t)tstart[t] * eb;
                 for (size_t off = 0; off < total; off += CH) {
                     size_t m = total - off < CH ? total - off : CH;
                     SG_CUDA(cudaMemcpy(buf.data(), src + off, m, cudaMemcpyDeviceToHost));
@@ -1408,16 +1515,24 @@ int snapgpu_index_save(const snapgpu_index *ix, const char *directory)
                 hashBytes += total;
             }
         }
-        fclose(f);
+        if (fclose(f) != 0) return sg_fail("snapgpu_index_save: cannot write GenomeIndexHash");
     }
     {
         FILE *f = fopen((dir + "/GenomeIndex").c_str(), "w");
         if (!f) return sg_fail("snapgpu_index_save: cannot write GenomeIndex");
-        fprintf(f, "%d %d %d %lld %d %d %d %lld %d %d", 7, 1, (int)ix->view.nTables, (long long)ix->view.overflowSize, (int)ix->view.seedLen,
-                (int)ix->view.chromosomePadding, (int)ix->view.keyBytes, (long long)hashBytes, ix->view.large ? 0 : 1, 4);
+        const std::string text = sg_genome_index_text(nT, ix->view.overflowSize, seedLen, ix->view.chromosomePadding, keyBytes, hashBytes, isLarge);
+        fputs(text.c_str(), f);
         fclose(f);
     }
     return 0;
+}
+
+int snapgpu_index_save(const snapgpu_index *ix, const char *directory)
+{
+    snapgpu_save_options o;
+    memset(&o, 0, sizeof(o));
+    o.struct_size = sizeof(o); o.keyBytes = 4; o.large = 0; o.slack = 0.3;
+    return snapgpu_index_save_ex(ix, directory, &o);
 }
 
 // ---- copies of an index on other devices of the same process (SURVEY 8e) ----
@@ -1463,6 +1578,7 @@ static int clone_alloc(const snapgpu_index *src, int device, snapgpu_index **out
     ix->h_tables_prob = src->h_tables_prob;
     ix->h_tableStart = src->h_tableStart; ix->h_tableSize = src->h_tableSize; ix->h_tableUsed = src->h_tableUsed;
     ix->h_contigStart = src->h_contigStart; ix->h_contigName = src->h_contigName; ix->h_contigIsAlt = src->h_contigIsAlt; ix->h_contigOriginal = src->h_contigOriginal;
+    ix->h_contigLines = src->h_contigLines;
     *out = ix;
     return 0;
 }

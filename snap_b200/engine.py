@@ -46,6 +46,19 @@ class PairedParams(C.Structure):
     ]
 
 
+class Contig(C.Structure):
+    """snapgpu_contig: one contig as the reference's Genome file holds it (name, location, ALT flag, original number, liftover)."""
+    _fields_ = [
+        ("name", C.c_char_p), ("beginningLocation", C.c_int64), ("isAlt", C.c_int32), ("originalContigNumber", C.c_int32),
+        ("projBeginningLocation", C.c_int64), ("projIsRC", C.c_int32), ("reserved", C.c_int32), ("projCigar", C.c_char_p),
+    ]
+
+
+class SaveOptions(C.Structure):
+    """snapgpu_save_options: the table geometry of a saved index (`snap-aligner index -keysize / -large / -h`)."""
+    _fields_ = [("struct_size", C.c_uint32), ("keyBytes", C.c_uint32), ("large", C.c_uint32), ("reserved", C.c_uint32), ("slack", C.c_double)]
+
+
 class IndexInfo(C.Structure):
     _fields_ = [
         ("countOfBases", C.c_int64), ("seedLen", C.c_uint32), ("hashTableKeySize", C.c_uint32),
@@ -80,7 +93,7 @@ N_COUNTERS = len(COUNTER_FIELDS) + 71
 # every symbol include/snapgpu.h declares
 EXPORTS = [
     "snapgpu_last_error", "snapgpu_abi_version", "snapgpu_device_count", "snapgpu_params_default",
-    "snapgpu_index_open", "snapgpu_index_build", "snapgpu_index_build_device", "snapgpu_index_save", "snapgpu_index_info_get", "snapgpu_index_close", "snapgpu_index_replicate", "snapgpu_host_alloc", "snapgpu_host_free",
+    "snapgpu_index_open", "snapgpu_index_build", "snapgpu_index_build_device", "snapgpu_index_build_genome", "snapgpu_index_build_genome_device", "snapgpu_index_save", "snapgpu_index_save_ex", "snapgpu_index_info_get", "snapgpu_index_close", "snapgpu_index_replicate", "snapgpu_host_alloc", "snapgpu_host_free",
     "snapgpu_group_create", "snapgpu_group_destroy", "snapgpu_group_size", "snapgpu_index_broadcast", "snapgpu_counters_allreduce",
     "snapgpu_lookup_seeds", "snapgpu_lookup_seeds_device", "snapgpu_measure_random_sector_rate", "snapgpu_aligner_create", "snapgpu_aligner_destroy", "snapgpu_align_single",
     "snapgpu_align_single_device", "snapgpu_align_single_secondary", "snapgpu_align_single_secondary_device", "snapgpu_paired_params_default", "snapgpu_paired_aligner_create", "snapgpu_align_paired",
@@ -88,7 +101,7 @@ EXPORTS = [
     "snapgpu_fastq_parse", "snapgpu_sam_create", "snapgpu_sam_destroy", "snapgpu_sam_format_single", "snapgpu_sam_format_paired", "snapgpu_sam_format_single_device", "snapgpu_sam_format_paired_device", "snapgpu_sam_set_format", "snapgpu_sam_header", "snapgpu_bgzf_device", "snapgpu_bgzf_deflate_device", "snapgpu_bam_index_members_device", "snapgpu_sam_sort_device", "snapgpu_sam_last_record_count", "snapgpu_bam_markdup_device", "snapgpu_bam_index_device", "snapgpu_aligner_launch_count", "snapgpu_test_lv", "snapgpu_test_ag", "snapgpu_test_lv_warp", "snapgpu_test_ag_warp",
 ]
 
-ABI_VERSION = 6          # include/snapgpu.h SNAPGPU_ABI_VERSION this mirror was written against
+ABI_VERSION = 7          # include/snapgpu.h SNAPGPU_ABI_VERSION this mirror was written against
 _lib = None
 
 
@@ -109,6 +122,10 @@ def lib():
         L.snapgpu_index_build.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int,
                                           C.POINTER(C.c_void_p)]
         L.snapgpu_index_build_device.argtypes = L.snapgpu_index_build.argtypes
+        L.snapgpu_index_build_genome.argtypes = [C.c_void_p, C.c_int64, C.POINTER(Contig), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int,
+                                                 C.POINTER(C.c_void_p)]
+        L.snapgpu_index_build_genome_device.argtypes = L.snapgpu_index_build_genome.argtypes
+        L.snapgpu_index_save_ex.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(SaveOptions)]
         L.snapgpu_lookup_seeds_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.snapgpu_index_save.argtypes = [C.c_void_p, C.c_char_p]
         L.snapgpu_index_info_get.argtypes = [C.c_void_p, C.POINTER(IndexInfo)]
@@ -237,6 +254,23 @@ class Index:
                                                 C.byref(h)))
         return Index(h, device)
 
+    @staticmethod
+    def build_genome(bases, contigs, seed_len: int = 20, chromosome_padding: int = 2000, device: int = 0, d_bases_ptr: int = 0) -> "Index":
+        """snapgpu_index_build_genome: padded bases (host array, or bases_ptr/n of device memory when d_bases_ptr is given) and one dict
+        per contig with the snapgpu_contig fields (name as bytes; projCigar bytes or None)."""
+        arr = (Contig * len(contigs))()
+        for i, c in enumerate(contigs):
+            for k, v in c.items():
+                setattr(arr[i], k, v)
+        h = C.c_void_p()
+        if d_bases_ptr:
+            _check(lib().snapgpu_index_build_genome_device(C.c_void_p(d_bases_ptr), int(bases), arr, len(contigs), seed_len, chromosome_padding,
+                                                           device, C.byref(h)))
+        else:
+            b = np.ascontiguousarray(bases, dtype=np.uint8)
+            _check(lib().snapgpu_index_build_genome(_p(b), b.size, arr, len(contigs), seed_len, chromosome_padding, device, C.byref(h)))
+        return Index(h, device)
+
     def lookup_seeds_device(self, d_seeds: int, n: int, d_nhits: int, d_hits: int = 0, d_probes: int = 0, max_hits: int = 0, stream: int = 0):
         _check(lib().snapgpu_lookup_seeds_device(self.handle, C.c_void_p(d_seeds), n, max_hits, C.c_void_p(d_nhits), C.c_void_p(d_hits),
                                                  C.c_void_p(d_probes), C.c_void_p(stream)))
@@ -250,6 +284,11 @@ class Index:
     def save(self, directory: str) -> None:
         """Writes a reference-format index directory (loadable by stock `snap-aligner`)."""
         _check(lib().snapgpu_index_save(self.handle, directory.encode()))
+
+    def save_ex(self, directory: str, key_bytes: int = 4, large: bool = False, slack: float = 0.3) -> None:
+        """Writes a reference-format index directory in the given table geometry (snapgpu_index_save_ex)."""
+        o = SaveOptions(C.sizeof(SaveOptions), key_bytes, 1 if large else 0, 0, slack)
+        _check(lib().snapgpu_index_save_ex(self.handle, directory.encode(), C.byref(o)))
 
     def info(self) -> IndexInfo:
         info = IndexInfo()
