@@ -22,10 +22,11 @@
 extern "C" {
 #endif
 
-#define SNAPGPU_ABI_VERSION 7   /* 2: snapgpu_sam_format_* take frontClipped / clippedLens before `results`; 3: groups, replicate, host_alloc, random-sector rate;
+#define SNAPGPU_ABI_VERSION 8   /* 2: snapgpu_sam_format_* take frontClipped / clippedLens before `results`; 3: groups, replicate, host_alloc, random-sector rate;
                                  * 4: snapgpu_sam_sort_device; 5: snapgpu_bam_markdup_device, snapgpu_bam_index_device;
                                  * 6: snapgpu_align_single_secondary(_device) (-om), snapgpu_bgzf_deflate_device, snapgpu_bam_index_members_device, snapgpu_sam_header;
-                                 * 7: snapgpu_contig, snapgpu_index_build_genome(_device), snapgpu_save_options, snapgpu_index_save_ex */
+                                 * 7: snapgpu_contig, snapgpu_index_build_genome(_device), snapgpu_save_options, snapgpu_index_save_ex;
+                                 * 8: snapgpu_aligner_deferred_count */
 
 /* AlignmentResult enum, reference SNAPLib/AlignmentResult.h:34 */
 enum { SNAPGPU_NOT_FOUND = 0, SNAPGPU_SINGLE_HIT = 1, SNAPGPU_MULTIPLE_HITS = 2 };
@@ -536,6 +537,9 @@ int  snapgpu_sam_format_paired_device(snapgpu_sam *s, int64_t nReads, uint32_t m
 
 /* Number of kernel launches issued through this aligner since creation (bench.py's gpu_launches). */
 int64_t snapgpu_aligner_launch_count(const snapgpu_aligner *a);
+/* Reads the last two-pass launch of a single-end aligner handed from its first pass to its second (affine-gap) pass; -1 for an aligner
+ * that has no two-pass launch (paired, or -ne).  Waits for the aligner's device to finish its work first. */
+int64_t snapgpu_aligner_deferred_count(snapgpu_aligner *a);
 
 /*
  * Leaf kernels exposed for parity tests (never used by the product path's callers).

@@ -386,8 +386,9 @@ struct SgCandScore {
 // HAM: the Hamming / gapless pass (AlignRead(..., useHamming = true)); a template parameter so that the stock pass carries none of its code.
 // DEFER: an instantiation WITHOUT the affine-gap code: at the point where the reference would rescore with affine gap it sets
 // A.deferred and unwinds; the caller then aligns that read again from scratch with the full instantiation (two-pass launch).
+// sg_score inlines this in the DEFER instantiation and calls the out-of-line sg_score_candidate below in the others (see there).
 template <bool HAM, bool DEFER>
-SG_HDN void sg_score_candidate(SgAligner &A, const SgElem &el, int64_t genomeLocationIn, int seedOffset, int scoreLimitForThisElement, SgCandScore *o)
+SG_HD void sg_score_candidate_inl(SgAligner &A, const SgElem &el, int64_t genomeLocationIn, int seedOffset, int scoreLimitForThisElement, SgCandScore *o)
 {
     const bool useHamming = HAM;
     const SgIndexView &ix = *A.ix; const SgParams &pr = *A.pr; const SgTables &T = *A.tb;
@@ -510,6 +511,16 @@ SG_HDN void sg_score_candidate(SgAligner &A, const SgElem &el, int64_t genomeLoc
     o->agScore = agScore;
 }
 
+// The call boundary of the full instantiations.  The first pass of the two-pass launch (DEFER, 40 registers at 6 CTAs per SM) does
+// without it: every candidate crossed it there, and the registers saved and restored around it went through the per-lane stack, which
+// every lane of the warp writes -- a 128-byte line per warp-uniform word.  Inlined, sg_align_kernel<6, 1> has a 624-byte frame instead
+// of 720 and takes 20.0 ms instead of 22.1 per 1 M-read step on an H100 SXM (700 W; DESIGN.md section 8).
+template <bool HAM, bool DEFER>
+SG_HDN void sg_score_candidate(SgAligner &A, const SgElem &el, int64_t genomeLocationIn, int seedOffset, int scoreLimitForThisElement, SgCandScore *o)
+{
+    sg_score_candidate_inl<HAM, DEFER>(A, el, genomeLocationIn, seedOffset, scoreLimitForThisElement, o);
+}
+
 // BaseAligner::score (:917-1534).  Returns true iff a result was reached.
 // SEC: the caller gave a secondaryResults buffer (`-om`): candidates within A.secMaxEditDist of the best are recorded as they are scored and the
 // "nothing can rescue MAPQ" stop (:1512) is off; an overflow of the buffer sets A.secOverflow and ends the read (the reference returns false
@@ -591,7 +602,8 @@ SG_HDN bool sg_score(SgAligner &A, bool forceResult, snapgpu_single_result *prim
                 bool genomeLocationIsNonALT = (!pr.altAwareness) || !A.isALT(genomeLocation);
 
                 SgCandScore cs;
-                sg_score_candidate<HAM, DEFER>(A, el, genomeLocation, (int)el.candSeedOffset[candidateIndexToScore], scoreLimitForThisElement, &cs);
+                if (DEFER) sg_score_candidate_inl<HAM, DEFER>(A, el, genomeLocation, (int)el.candSeedOffset[candidateIndexToScore], scoreLimitForThisElement, &cs);
+                else sg_score_candidate<HAM, DEFER>(A, el, genomeLocation, (int)el.candSeedOffset[candidateIndexToScore], scoreLimitForThisElement, &cs);
                 if (DEFER && A.deferred) return true;
                 unsigned score = cs.score;
                 double matchProbability = cs.matchProbability;

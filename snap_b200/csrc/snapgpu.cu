@@ -3789,6 +3789,15 @@ int snapgpu_fastq_parse(snapgpu_fastq *f, const char *text, int64_t nBytes, int 
 
 int64_t snapgpu_aligner_launch_count(const snapgpu_aligner *a) { return a ? a->launches : 0; }
 
+int64_t snapgpu_aligner_deferred_count(snapgpu_aligner *a)
+{
+    if (!a || a->paired || !a->twoPass || !a->d_retryCount) return -1;
+    unsigned long long v = 0;
+    if (cudaSetDevice(a->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
+        cudaMemcpy(&v, a->d_retryCount, 8, cudaMemcpyDeviceToHost) != cudaSuccess) { sg_fail(cudaGetErrorString(cudaGetLastError())); return -1; }
+    return (int64_t)v;
+}
+
 static int leaf_scratch(int device, SgParams *p, int *threads, uint8_t **d_scratch, size_t *bytes, SgTables **d_tb)
 {
     if (require_device(device)) return 1;

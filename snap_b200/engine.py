@@ -98,10 +98,10 @@ EXPORTS = [
     "snapgpu_lookup_seeds", "snapgpu_lookup_seeds_device", "snapgpu_measure_random_sector_rate", "snapgpu_aligner_create", "snapgpu_aligner_destroy", "snapgpu_align_single",
     "snapgpu_align_single_device", "snapgpu_align_single_secondary", "snapgpu_align_single_secondary_device", "snapgpu_paired_params_default", "snapgpu_paired_aligner_create", "snapgpu_align_paired",
     "snapgpu_align_paired_device", "snapgpu_aligner_check", "snapgpu_fastq_create", "snapgpu_fastq_destroy", "snapgpu_fastq_parse_device",
-    "snapgpu_fastq_parse", "snapgpu_sam_create", "snapgpu_sam_destroy", "snapgpu_sam_format_single", "snapgpu_sam_format_paired", "snapgpu_sam_format_single_device", "snapgpu_sam_format_paired_device", "snapgpu_sam_set_format", "snapgpu_sam_header", "snapgpu_bgzf_device", "snapgpu_bgzf_deflate_device", "snapgpu_bam_index_members_device", "snapgpu_sam_sort_device", "snapgpu_sam_last_record_count", "snapgpu_bam_markdup_device", "snapgpu_bam_index_device", "snapgpu_aligner_launch_count", "snapgpu_test_lv", "snapgpu_test_ag", "snapgpu_test_lv_warp", "snapgpu_test_ag_warp",
+    "snapgpu_fastq_parse", "snapgpu_sam_create", "snapgpu_sam_destroy", "snapgpu_sam_format_single", "snapgpu_sam_format_paired", "snapgpu_sam_format_single_device", "snapgpu_sam_format_paired_device", "snapgpu_sam_set_format", "snapgpu_sam_header", "snapgpu_bgzf_device", "snapgpu_bgzf_deflate_device", "snapgpu_bam_index_members_device", "snapgpu_sam_sort_device", "snapgpu_sam_last_record_count", "snapgpu_bam_markdup_device", "snapgpu_bam_index_device", "snapgpu_aligner_launch_count", "snapgpu_aligner_deferred_count", "snapgpu_test_lv", "snapgpu_test_ag", "snapgpu_test_lv_warp", "snapgpu_test_ag_warp",
 ]
 
-ABI_VERSION = 7          # include/snapgpu.h SNAPGPU_ABI_VERSION this mirror was written against
+ABI_VERSION = 8          # include/snapgpu.h SNAPGPU_ABI_VERSION this mirror was written against
 _lib = None
 
 
@@ -175,6 +175,8 @@ def lib():
         L.snapgpu_fastq_parse_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int] + [C.c_void_p] * 7 + [C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p]
         L.snapgpu_aligner_launch_count.restype = C.c_int64
         L.snapgpu_aligner_launch_count.argtypes = [C.c_void_p]
+        L.snapgpu_aligner_deferred_count.restype = C.c_int64
+        L.snapgpu_aligner_deferred_count.argtypes = [C.c_void_p]
         L.snapgpu_test_lv.argtypes = [C.c_int, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int64, C.c_void_p]
         L.snapgpu_test_ag.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
                                       C.c_int64, C.c_void_p]
@@ -399,6 +401,10 @@ class SingleAligner:
 
     def launch_count(self) -> int:
         return int(lib().snapgpu_aligner_launch_count(self.handle))
+
+    def deferred_count(self) -> int:
+        """Reads the last two-pass launch sent on to its affine-gap pass (-1 without a two-pass launch); waits for the device."""
+        return int(lib().snapgpu_aligner_deferred_count(self.handle))
 
     def close(self):
         if self.handle:
