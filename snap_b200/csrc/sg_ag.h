@@ -7,6 +7,15 @@
 // int16 saturation except the INT16_MIN padding profile, which is handled explicitly.
 #pragma once
 #include "sg_common.h"
+
+// Counting points of the scalar form (tools/narrow_band_counts.py defines them; empty everywhere else): one call, and one
+// (row, segment) unit with the number of lazy-F rounds it entered.
+#ifndef SG_AG_CALL_HOOK
+#define SG_AG_CALL_HOOK(banded, numVec, w, patternLen, textLen)
+#endif
+#ifndef SG_AG_UNIT_HOOK
+#define SG_AG_UNIT_HOOK(row, seg, nVecHere, rounds) ((void)(rounds))
+#endif
 #include "sg_seed.h"
 
 struct SgAgParams {
@@ -302,6 +311,7 @@ SG_HDN void sg_ag_compute(const SgTables &T, const SgScratch &S, const SgAgParam
     lay.w = w; lay.patternLen = patternLen;
     const int numVec = lay.numVec, segLen = lay.segLen, numSeg = lay.numSeg;
     const int stride = lay.rowStride();
+    SG_AG_CALL_HOOK(banded, numVec, w, patternLen, textLen);
 
     int endBonus;                    // :950-966
     if (!isRC) endBonus = (dir == -1) ? P.fivePrimeEndBonus : P.threePrimeEndBonus;
@@ -388,13 +398,15 @@ SG_HDN void sg_ag_compute(const SgTables &T, const SgScratch &S, const SgAgParam
             }
 
             // lazy F
-            int passes = banded ? (SG_VEC - 1) : SG_VEC;
+            int passes = banded ? (SG_VEC - 1) : SG_VEC, rounds = 0;
             for (int kk = 0; kk < passes; kk++) {
+                rounds++;
                 if (banded) { if (f[SG_VEC - 1] > X[0]) X[0] = f[SG_VEC - 1]; }   // X = max(X, f >> 7 lanes) (:537)
                 for (int l = SG_VEC - 1; l > 0; l--) f[l] = f[l - 1];
                 f[0] = 0;
                 if (sg_ag_lazy_pass(P, Hm1ptr, btRow, j * numVec, nVecHere, f, maxv)) break;
             }
+            SG_AG_UNIT_HOOK(i, j, nVecHere, rounds);
             if (banded) { for (int l = 0; l < SG_VEC; l++) f[l] = X[l]; }          // pass f on to the next segment (:572)
         }
 

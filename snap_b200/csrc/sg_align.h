@@ -387,7 +387,8 @@ struct SgCandScore {
 // DEFER: an instantiation WITHOUT the affine-gap code: at the point where the reference would rescore with affine gap it sets
 // A.deferred and unwinds; the caller then aligns that read again from scratch with the full instantiation (two-pass launch).
 // sg_score inlines this in the DEFER instantiation and calls the out-of-line sg_score_candidate below in the others (see there).
-template <bool HAM, bool DEFER>
+// AGM: the affine-gap forms the kernel carries (sg_warp_ag_compute); 1 in the second pass of the two-pass launch.
+template <bool HAM, bool DEFER, int AGM = 0>
 SG_HD void sg_score_candidate_inl(SgAligner &A, const SgElem &el, int64_t genomeLocationIn, int seedOffset, int scoreLimitForThisElement, SgCandScore *o)
 {
     const bool useHamming = HAM;
@@ -466,8 +467,8 @@ SG_HD void sg_score_candidate_inl(SgAligner &A, const SgElem &el, int64_t genome
                 if (tailStart != readLen) {
                     int patternLen = readLen - tailStart;
                     bool banded = (patternLen >= (3 * (2 * scoreLimitForThisElement + 1))) && !pr.noBandedAffineGap;
-                    sg_ag_dispatch(T, A.sc, A.ag, 1, banded, data + tailStart, textLen, readToScore + tailStart, qualToScore + tailStart,
-                                   patternLen, scoreLimitForThisElement, readLen, dirn != 0, false, &ar, sg_lane());
+                    sg_ag_dispatch<AGM>(T, A.sc, A.ag, 1, banded, data + tailStart, textLen, readToScore + tailStart, qualToScore + tailStart,
+                                        patternLen, scoreLimitForThisElement, readLen, dirn != 0, false, &ar, sg_lane());
                     agScore1 = ar.agScore; basesClippedAfter = ar.patternOffset; score1 = ar.nEdits; matchProb1 = ar.matchProbability;
                     agScore1 += (seedLen - readLen);
                 }
@@ -477,8 +478,8 @@ SG_HD void sg_score_candidate_inl(SgAligner &A, const SgElem &el, int64_t genome
                         int patternLen = seedOffset;
                         bool banded = (patternLen >= (3 * (2 * limitLeft + 1))) && !pr.noBandedAffineGap;
                         ar.textOffset = genomeLocationOffset; ar.patternOffset = basesClippedBefore; ar.matchProbability = matchProb2;
-                        sg_ag_dispatch(T, A.sc, A.ag, -1, banded, data + seedOffset, seedOffset + limitLeft, revRead + readLen - seedOffset,
-                                       oppQual + readLen - seedOffset, seedOffset, limitLeft, readLen, dirn != 0, false, &ar, sg_lane());
+                        sg_ag_dispatch<AGM>(T, A.sc, A.ag, -1, banded, data + seedOffset, seedOffset + limitLeft, revRead + readLen - seedOffset,
+                                            oppQual + readLen - seedOffset, seedOffset, limitLeft, readLen, dirn != 0, false, &ar, sg_lane());
                         agScore2 = ar.agScore; genomeLocationOffset = ar.textOffset; basesClippedBefore = ar.patternOffset;
                         score2 = ar.nEdits; matchProb2 = ar.matchProbability;
                         agScore2 -= readLen;
@@ -515,17 +516,17 @@ SG_HD void sg_score_candidate_inl(SgAligner &A, const SgElem &el, int64_t genome
 // without it: every candidate crossed it there, and the registers saved and restored around it went through the per-lane stack, which
 // every lane of the warp writes -- a 128-byte line per warp-uniform word.  Inlined, sg_align_kernel<6, 1> has a 624-byte frame instead
 // of 720 and takes 20.0 ms instead of 22.1 per 1 M-read step on an H100 SXM (700 W; DESIGN.md section 8).
-template <bool HAM, bool DEFER>
+template <bool HAM, bool DEFER, int AGM = 0>
 SG_HDN void sg_score_candidate(SgAligner &A, const SgElem &el, int64_t genomeLocationIn, int seedOffset, int scoreLimitForThisElement, SgCandScore *o)
 {
-    sg_score_candidate_inl<HAM, DEFER>(A, el, genomeLocationIn, seedOffset, scoreLimitForThisElement, o);
+    sg_score_candidate_inl<HAM, DEFER, AGM>(A, el, genomeLocationIn, seedOffset, scoreLimitForThisElement, o);
 }
 
 // BaseAligner::score (:917-1534).  Returns true iff a result was reached.
 // SEC: the caller gave a secondaryResults buffer (`-om`): candidates within A.secMaxEditDist of the best are recorded as they are scored and the
 // "nothing can rescue MAPQ" stop (:1512) is off; an overflow of the buffer sets A.secOverflow and ends the read (the reference returns false
 // from AlignRead and its caller starts over with a larger buffer, SingleAligner.cpp:250-263).
-template <bool HAM, bool DEFER, bool SEC = false>
+template <bool HAM, bool DEFER, bool SEC = false, int AGM = 0>
 SG_HDN bool sg_score(SgAligner &A, bool forceResult, snapgpu_single_result *primaryResult)
 {
     const bool useHamming = HAM;
@@ -603,7 +604,7 @@ SG_HDN bool sg_score(SgAligner &A, bool forceResult, snapgpu_single_result *prim
 
                 SgCandScore cs;
                 if (DEFER) sg_score_candidate_inl<HAM, DEFER>(A, el, genomeLocation, (int)el.candSeedOffset[candidateIndexToScore], scoreLimitForThisElement, &cs);
-                else sg_score_candidate<HAM, DEFER>(A, el, genomeLocation, (int)el.candSeedOffset[candidateIndexToScore], scoreLimitForThisElement, &cs);
+                else sg_score_candidate<HAM, DEFER, AGM>(A, el, genomeLocation, (int)el.candSeedOffset[candidateIndexToScore], scoreLimitForThisElement, &cs);
                 if (DEFER && A.deferred) return true;
                 unsigned score = cs.score;
                 double matchProbability = cs.matchProbability;
@@ -784,7 +785,7 @@ SG_HDN void sg_finalize_secondary(SgAligner &A, snapgpu_single_result *primaryRe
 
 // BaseAligner::AlignRead (:272-763) for one read with the stock loop's arguments (SingleAligner.cpp:250).
 // `result` must be caller-zeroed POD; on return it holds what the reference would have put in primaryResult.
-template <bool HAM, bool DEFER = false, bool SEC = false>
+template <bool HAM, bool DEFER = false, bool SEC = false, int AGM = 0>
 SG_HDN void sg_align_read_t(SgAligner &A, const uint8_t *readData, const uint8_t *readQuality, uint32_t readLen, snapgpu_single_result *primaryResult)
 {
     const SgIndexView &ix = *A.ix; const SgParams &pr = *A.pr; const SgTables &T = *A.tb;
@@ -887,7 +888,7 @@ SG_HDN void sg_align_read_t(SgAligner &A, const uint8_t *readData, const uint8_t
         if (nextSeedToTest >= nPossibleSeeds) {
             A.wrapCount++;
             if (A.wrapCount >= seedLen) {
-                sg_score<HAM, DEFER, SEC>(A, true, primaryResult);
+                sg_score<HAM, DEFER, SEC, AGM>(A, true, primaryResult);
                 primaryResult->scorePriorToClipping = primaryResult->score;     // finalizeSecondaryResults, :2442
                 if (SEC && !A.secOverflow) sg_finalize_secondary(A, primaryResult);
                 return;
@@ -969,14 +970,14 @@ SG_HDN void sg_align_read_t(SgAligner &A, const uint8_t *readData, const uint8_t
         nextSeedToTest += seedLen;
 
         if (appliedEitherSeed) {
-            if (sg_score<HAM, DEFER, SEC>(A, false, primaryResult)) {
+            if (sg_score<HAM, DEFER, SEC, AGM>(A, false, primaryResult)) {
                 primaryResult->scorePriorToClipping = primaryResult->score;
                 if (SEC && !A.secOverflow) sg_finalize_secondary(A, primaryResult);
                 return;
             }
         }
     }
-    sg_score<HAM, DEFER, SEC>(A, true, primaryResult);
+    sg_score<HAM, DEFER, SEC, AGM>(A, true, primaryResult);
     primaryResult->scorePriorToClipping = primaryResult->score;
     if (SEC && !A.secOverflow) sg_finalize_secondary(A, primaryResult);
 }

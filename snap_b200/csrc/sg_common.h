@@ -95,6 +95,7 @@ struct SgParams {
     uint32_t tableSlots;             // power of two >= 2*poolSize (our candidate lookup table)
     uint32_t maxReadLen;             // scratch sizing bound
     int32_t  agSpecialised;          // device tuning knob (no effect on results): SgAgParams.usePacked of the single-end kernel's second pass
+                                     // (+ 4: its bands of up to 32 columns take the two-unit form, SNAPGPU_SINGLE_AG_NARROW)
     uint32_t tmaMinHits;             // device tuning knob (no effect on results): hit lists of at least this many locations are staged through shared memory with bulk copies; 0 = never
 };
 
@@ -135,8 +136,7 @@ struct SgScratch {
     int16_t  *agProf;                // [5*agCols] striped query profile of the current affine-gap call (device warp forms): int16 per cell in
                                      // every form, as the reference keeps it (the packed forms pair two cells as s16x2)
     uint32_t agCols, agRows;
-    uint32_t *agSnap;                // [7*32] H after each lazy-F round of the experimental narrow-band form (sg_warp_ag_duo.cuh): shared memory
-                                     // where the kernel has a block for it, NULL = the Landau-Vishkin cell array of the arena (idle during an affine-gap call)
+    uint32_t *agSnap;                // unused: an earlier narrow-band form kept its per-round H here; the SIMT emulator of the CPU suite still sets it
     // Small copies in SHARED memory (the alignment kernels set them per warp; NULL / 0 elsewhere): Landau-Vishkin needs (k+1)(2k+1)
     // cells of L and A for the k it is called with and k+1 backtrace entries -- a few hundred bytes at the usual k <= 15 -- and
     // arrays that small must not live in (and be written back to) HBM.

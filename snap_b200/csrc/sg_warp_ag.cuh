@@ -159,8 +159,11 @@ __device__ __noinline__ void sg_warp_ag_rows_banded4(const SgScratch &S, int ope
 }
 
 
-// AGM: 2 = the caller's kernel may take the unrolled packed instantiation (only stage 2 of the paired launch carries that code);
-//      3 = 2 + the experimental narrow-band form of sg_warp_ag_duo.cuh when SgAgParams.usePacked has bit 2 set (leaf tests only)
+// AGM, the forms the caller's kernel carries beyond the general, packed and banded4 ones (bits, so that no other kernel grows):
+//      1 = the two-unit narrow-band form of sg_warp_ag_duo.cuh, taken when SgAgParams.usePacked has bit 2 set (the single-end second
+//          pass, SNAPGPU_SINGLE_AG_NARROW=duo);
+//      2 = the unrolled packed instantiation (stage 2 of the paired launch);
+//      3 = both (the leaf-test kernel and the SIMT emulator of the CPU suite)
 template <int AGM = 0>
 __device__ __noinline__ void sg_warp_ag_compute(const SgTables &T, const SgScratch &S, const SgAgParams &P, int dir, bool banded,
                                                 const uint8_t *text, int textLen, const uint8_t *pattern, const uint8_t *quality, int patternLen,
@@ -221,18 +224,17 @@ __device__ __noinline__ void sg_warp_ag_compute(const SgTables &T, const SgScrat
         // unbanded, up to 192 columns: the packed (two cells per lane, DPX s16x2) register-resident form
         __syncwarp();
         SgAgBests bb;
-        if (AGM >= 2 && (P.usePacked & 3) == 2) sg_warp_ag_rows_packed<true>(S, P, dir, text, textLen, pattern, patternLen, scoreInit, lay, bt, lane, &bb);
+        if ((AGM & 2) && (P.usePacked & 3) == 2) sg_warp_ag_rows_packed<true>(S, P, dir, text, textLen, pattern, patternLen, scoreInit, lay, bt, lane, &bb);
         else sg_warp_ag_rows_packed<false>(S, P, dir, text, textLen, pattern, patternLen, scoreInit, lay, bt, lane, &bb);
         sg_ag_finish(T, P, lay, bt, dir, text, pattern, quality, patternLen, scoreInit, endBonus, useClippingOptimizations,
                      bb.lScore, bb.lText, bb.lPat, bb.gScore, bb.gText, out);
         return;
     }
 #endif
-    if (AGM == 3 && banded && numVec <= 4 && (P.usePacked & 3) && (P.usePacked & 4)) {
-        // bands of up to 32 columns, the experimental form: two (row, segment) units per step, two cells per lane, lazy F without
-        // its loop (sg_warp_ag_duo.cuh).  Same results; 12 % fewer instructions than the one-cell-per-lane form below but 4 % slower
-        // in the single-end kernel and 10 % in the paired one (instruction-fetch stalls: its step is 530 instructions of straight-line
-        // code against a 6 KB L0), so only the leaf-test kernel (AGM 3) and the SIMT emulator of the CPU suite instantiate it.
+    if ((AGM & 1) && banded && numVec <= 4 && (P.usePacked & 3) && (P.usePacked & 4)) {
+        // bands of up to 32 columns: two (row, segment) units per step, two cells per lane (sg_warp_ag_duo.cuh).  Same results as
+        // sg_warp_ag_rows_banded4 below; slower than it on H100 (DESIGN.md section 8), so the second pass takes it only under
+        // SNAPGPU_SINGLE_AG_NARROW=duo.
         __syncwarp();
         SgAgBests bb;
         sg_warp_ag_rows_banded_duo(S, P, dir, text, textLen, pattern, patternLen, w, scoreInit, lay, bt, lane, &bb);

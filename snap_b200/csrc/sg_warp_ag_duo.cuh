@@ -1,5 +1,6 @@
 // sg_warp_ag_duo.cuh -- the banded affine-gap DP for bands of up to 32 columns (numVec <= 4: every `snap single -d 14` rescoring),
-// two (row, segment) units per step, two cells per lane as s16x2 on the DPX min/max unit, and the lazy-F rounds without a loop.
+// two (row, segment) units per step, two cells per lane as s16x2 on the DPX min/max unit.  The single-end second pass takes it under
+// SNAPGPU_SINGLE_AG_NARROW=duo; the leaf-test kernel and the SIMT emulator of the CPU suite under SgAgParams.usePacked bit 2.
 //
 // A band of 2w+1 <= segLen columns touches at most two of the reference's segments in a row, and the reference computes both
 // whole (AffineGapVectorized.h:256-819: vectors 0 .. nVecHere-1 of every segment between the one holding the band's first column and
@@ -17,11 +18,12 @@
 // sg_warp_ag_rows_banded4 and therefore as the reference; the only cell two concurrent units share -- the previous row's last
 // cell of segment j, read by (i, j+1) and overwritten by (i+1, j) -- is read before the step's writes.
 //
-// Counted on one step of `snap single -d 14`: the one-cell-per-lane form enters its lazy-F loop 60.7 M
-// times and runs 270 M rounds of it (4.4 per unit: with gap-extend 1 against gap-open 7 the cells right of the diagonal stay
-// within reach of F), a third of the kernel's instructions; a two-unit step whose halves vote round by round runs the LONGER of
-// its two loops (6.3 rounds per step) and loses what the packing wins.  Hence the loop-free form below: all 7 rounds evaluated
-// branch-free, one reduction to find where the reference would have stopped.
+// The lazy-F loop (4.4 rounds per unit on `snap single -d 14`: with gap-extend 1 against gap-open 7 the cells right of the
+// diagonal stay within reach of F) runs once per step for both units, as long as the longer of the two (6.3 rounds per step), and
+// commits as it goes like banded4's.  Every loop is `#pragma unroll 1`: the kernel is instruction-fetch bound, and a step of
+// straight-line code (7 rounds evaluated and reduced at the end, as an earlier form of this function did) outgrows the L0 cache.
+// Counted on `snap single -d 14` (tools/narrow_band_counts.py): 0.61 steps per banded4 unit, but at 64 registers the step spills
+// (~360 instructions outside the loop, 47 per round, against banded4's ~185 per unit and 28 per round), so it is not faster.
 #pragma once
 
 __device__ __noinline__ void sg_warp_ag_rows_banded_duo(const SgScratch &S, const SgAgParams &P, int dir, const uint8_t *text, int textLen,
@@ -36,8 +38,6 @@ __device__ __noinline__ void sg_warp_ag_rows_banded_duo(const SgScratch &S, cons
     const int open = P.gapOpenPenalty, ext = P.gapExtendPenalty;
     const unsigned nOpen2 = sg_pk2(-open), nExt2 = sg_pk2(-ext), nQExt2 = sg_pk2(-q * ext);
     const unsigned aMask = (a == 0) ? 0xffff0000u : 0xffffffffu;       // SSE lane 0 takes 0 when f moves up a lane
-    // H after each lazy-F round, [round][lane]: shared memory when the kernel has a block for it, else an (idle) array of the arena
-    unsigned *snap = ((S.agSnap != (uint32_t *)0) ? S.agSnap : (uint32_t *)S.lvL) + lane;
     unsigned *prof = (unsigned *)S.agProf;               // [5][strideW] packed substitution scores of the pattern columns
 
     for (int x = lane; x < strideW; x += 32) {
@@ -130,56 +130,49 @@ __device__ __noinline__ void sg_warp_ag_rows_banded_duo(const SgScratch &S, cons
         // f register of the SSE lanes after the main pass (the same in all four vectors' lanes)
         const unsigned fl0 = __vimax_s16x2_relu((nVecHere == 1) ? p1 : (nVecHere == 2) ? p2 : (nVecHere == 3) ? p3 : p4, 0u);
 
-        // ---------------- lazy F (:534-569) without its loop ----------------
+        // ---------------- lazy F (:534-569), both halves' units in one loop ----------------
         // The reference runs up to 7 rounds (f moves up one SSE lane and decays by nVecHere*ext per round) over the vectors in
         // order, updating H and the traceback bits, and stops after the first (round, vector) in which no lane can still change a
-        // later cell.  With gap-extend 1 against gap-open 7 the cells right of the alignment's diagonal stay within reach of F
-        // round after round, so most units run many rounds, each with its own vote.  Here all 7 rounds are evaluated
-        // back to back as if none stopped -- H after each round kept in the warp's shared-memory block, "live" flags
-        // gathered in two bit sets (bit 4*round + vector, one set per cell of the word) -- then ONE reduction over the half
-        // finds the stop (first missing bit, in the reference's round-major order) and every lane takes H, the bits and X from
-        // the rounds that really ran.
-        const unsigned qBits = 0x1111111u << q;
+        // later cell.  One ballot per round carries both halves' live lanes (bit half*16 + q*4 + a); per half, the lowest all-zero
+        // nibble is the first vector with no live lane, and a lane commits the round only if its vector is at or before it -- the
+        // rule of sg_warp_ag_rows_banded4, a nibble per vector instead of a byte.  A vector outside its half's unit votes live
+        // (`fill`), so it never stops the loop.  A half that has stopped, or has no unit, commits nothing more; the loop ends when
+        // both halves have stopped.  A lane commits rounds 0 .. k-1 and no later one, so H only grows and the bits are taken
+        // after the loop: 2 if H grew, 32 if f - ext beat H - open in a committed round (liveAcc > 0).
         const unsigned nD2 = sg_pk2(-nVecHere * ext);
-        unsigned accLo = valid ? 0u : qBits, accHi = accLo;      // a vector outside the unit counts as live: it never stops the loop
-        unsigned h = hMain, fl = fl0;
-        {
-            // (not unrolled: the kernel is instruction-fetch bound, and 7 copies of the round do not fit the L0 instruction cache
-            //  next to the rest of the step -- unrolled it was slower than the one-cell-per-lane form it replaces)
-            unsigned bit = 1u << q;
-            unsigned *sp = snap;
-            #pragma unroll 1
-            for (int kk = 0; kk < SG_VEC - 1; kk++) {
-                const unsigned below = __shfl_up_sync(FULL, fl, 1);
-                const unsigned flS = __byte_perm(fl, below, 0x1076) & aMask;                  // f = f << one SSE lane
-                bool lgeHi, lgeLo;
-                const unsigned fv = __viaddmax_s16x2_relu(flS, nQExt2, 0u);
-                h = __vmaxs2(h, fv);                                                          // f > h: take it
-                *sp = h;
-                const unsigned tmp2 = __viaddmax_s16x2_relu(h, nOpen2, 0u);
-                const unsigned fn = __viaddmax_s16x2_relu(fv, nExt2, 0u);
-                (void)__vibmax_s16x2(tmp2, fn, &lgeHi, &lgeLo);                               // live: f - ext > h - open
-                if (!lgeLo) accLo |= bit;
-                if (!lgeHi) accHi |= bit;
-                fl = __viaddmax_s16x2_relu(flS, nD2, 0u);
-                bit <<= 4; sp += 32;
-            }
-        }
-        // (two full-warp reductions, each fed by one half: a reduction over a sub-warp mask that differs between the halves takes the
-        //  compiler's out-of-line divergent path -- REDUX writes ONE uniform register per warp)
-        const unsigned live0 = __reduce_or_sync(FULL, half ? 0u : (accLo | accHi)), live1 = __reduce_or_sync(FULL, half ? (accLo | accHi) : 0u);
-        const unsigned liveAll = half ? live1 : live0;
-        const unsigned dead = ~liveAll & 0x0fffffffu;
-        const int stop = dead ? (__ffs(dead) - 1) : 28;                                       // 4 * round + vector of the stop
-        const int nExec = dead ? (stop >> 2) + 1 : 7;                                         // rounds entered
-        const int nMine = dead ? (stop >> 2) + (q <= (stop & 3) ? 1 : 0) : 7;                 // rounds that updated my vector
+        // Every read of the rows in memory (hInit above all, see the header) before any write of this step.  Without this barrier,
+        // and with bit 32 taken by a DPX max against 0 after the loop, the device gave other results than the SIMT emulator on ~3 % of
+        // narrow-band jobs (tests/test_gpu_scoring_schemes.py, form 5); with both changes the two agree.
         __syncwarp();
-        if (nMine > 0) h = snap[(nMine - 1) * 32]; else h = hMain;
+        const unsigned fill = ~__ballot_sync(FULL, valid);
+        const unsigned myHalf = half ? 0x88880000u : 0x00008888u;
+        const unsigned beforeMe = (0x8888u & ((1u << (4 * q)) - 1u)) << (16 * half);    // nibble tops of my half's vectors before mine
+        unsigned seen = ((fill & 0xffffu) == 0xffffu ? 0x8u : 0u) | ((fill >> 16) == 0xffffu ? 0x80000u : 0u);   // halves stopped
+        bool stopped = (seen & myHalf) != 0u;
+        unsigned h = hMain, fl = fl0, liveAcc = 0u;
+        int nExec = SG_VEC - 1;                                  // rounds my half entered
+        #pragma unroll 1
+        for (int kk = 0; kk < SG_VEC - 1; kk++) {
+            const unsigned below = __shfl_up_sync(FULL, fl, 1);
+            const unsigned flS = __byte_perm(fl, below, 0x1076) & aMask;                  // f = f << one SSE lane
+            const unsigned fv = __viaddmax_s16x2_relu(flS, nQExt2, 0u);
+            const unsigned newh = __vmaxs2(h, fv);                                        // f > h: take it
+            const unsigned tmp2 = __viaddmax_s16x2_relu(newh, nOpen2, 0u);
+            const unsigned fn = __viaddmax_s16x2_relu(fv, nExt2, 0u);
+            bool lgeHi, lgeLo;
+            (void)__vibmax_s16x2(tmp2, fn, &lgeHi, &lgeLo);                               // live: f - ext > h - open
+            const unsigned vote = __ballot_sync(FULL, !(lgeLo && lgeHi)) | fill;
+            const unsigned zb = __vsub2(vote, 0x11111111u) & ~vote & 0x88888888u;         // (no borrow between the halves)
+            if (!stopped && !(zb & beforeMe)) { h = newh; liveAcc = __vmaxs2(liveAcc, __vsub2(fn, tmp2)); }
+            if (!stopped && (zb & myHalf)) { stopped = true; nExec = kk + 1; }
+            seen |= zb;
+            if ((seen & 0xffffu) && (seen >> 16)) break;
+            fl = __viaddmax_s16x2_relu(flS, nD2, 0u);
+        }
         {
-            const unsigned ran = qBits & ((nMine >= 7) ? 0x0fffffffu : ((1u << (4 * nMine)) - 1u));
             bool geHi, geLo;
-            (void)__vibmax_s16x2(hMain, h, &geHi, &geLo);                                      // bit 2: some round's f beat H
-            act |= ((geLo ? 0u : 2u) | ((accLo & ran) ? 32u : 0u)) | (((geHi ? 0u : 2u) | ((accHi & ran) ? 32u : 0u)) << 8);
+            (void)__vibmax_s16x2(hMain, h, &geHi, &geLo);                                  // bit 2: some round's f beat H
+            act |= ((geLo ? 0u : 2u) | ((liveAcc & 0xffffu) ? 32u : 0u)) | (((geHi ? 0u : 2u) | ((liveAcc >> 16) ? 32u : 0u)) << 8);   // bit 32
         }
         // X (:572): the largest value lane 7 held at the top of a round that was entered = SSE lane 7-r's f, r rounds decayed
         {

@@ -384,6 +384,8 @@ sg_align_kernel(const __grid_constant__ SgIndexView ixParam, const __grid_consta
                 A.work = workBefore;
                 continue;
             }
+        } else if (MODE == 2) {
+            sg_align_read_t<false, false, false, 1>(A, rd, rq, len, &r);     // (AGM 1: with the two-unit narrow-band form)
         } else {
             sg_align_read(A, rd, rq, len, &r);
         }
@@ -790,8 +792,8 @@ __global__ void sg_test_ag_warp_kernel(const SgTables *tb, SgParams pr, SgAgPara
     long long nW = ((long long)gridDim.x * blockDim.x) >> 5;
     SgScratch s;
     sg_scratch_carve(pr, scratchBase + (size_t)wid * scratchBytes, &s);
-    __shared__ uint32_t snapS[7 * 32];           // (one warp per block)
-    if (!(P.usePacked & 8)) s.agSnap = snapS;    // usePacked & 4: the experimental narrow-band form; & 8: with its per-round H in the arena
+    // usePacked & 4: the two-unit narrow-band form.  & 8 once put that form's per-round H in the arena instead of shared memory; the
+    // looped form keeps no per-round H, so 8 now runs the same form (the tests still name both)
     for (long long j = wid; j < nJobs; j += nW) {
         SgAgResult r;
         r.agScore = -1; r.textOffset = 0; r.patternOffset = 0; r.nEdits = 0; r.matchProbability = 0.0;
@@ -1977,6 +1979,15 @@ int snapgpu_aligner_create(const snapgpu_index *idx, const snapgpu_params *param
     // candidate is rescored) ; without affine gap at all the first pass simply finishes everything.  SNAPGPU_TWO_PASS=0 turns it off.
     a->params.agSpecialised = 1;         // second pass: narrow-band / packed affine-gap forms (faster there; they cost throughput in the one-launch form)
     if (const char *e = getenv("SNAPGPU_SINGLE_AG_SPECIALISED")) a->params.agSpecialised = atoi(e);       // 0 off, 1 on, 2 on with the unrolled packed form
+    // bands of up to 32 columns in the second pass: `rows` (default) one (row, segment) unit per warp step (sg_warp_ag_rows_banded4),
+    // `duo` two per step (sg_warp_ag_duo.cuh).  Same results; on `snap single -d 14` on an H100 the second pass takes 41.7 ms with
+    // `rows` and 46.9 ms with `duo` (DESIGN.md section 6).
+    {
+        const char *e = getenv("SNAPGPU_SINGLE_AG_NARROW");
+        const bool duo = e && strcmp(e, "duo") == 0;
+        if (e && !duo && strcmp(e, "rows") != 0) { snapgpu_aligner_destroy(a); return sg_fail("SNAPGPU_SINGLE_AG_NARROW must be rows or duo"); }
+        if (duo) a->params.agSpecialised |= 4;
+    }
     a->params.tmaMinHits = 0;            // hit-list staging through shared memory (bulk copies): off by default, not measured on H100
     if (const char *e = getenv("SNAPGPU_TMA_MIN_HITS")) a->params.tmaMinHits = (uint32_t)atoi(e);
     a->twoPass = !a->params.noEditDistance;

@@ -3,10 +3,12 @@
 batch size): the first pass (sg_align_kernel<., 1>), the second (affine-gap) pass (sg_align_kernel<., 2>), the whole step, and the
 number of reads the first pass deferred to the second.  Prints one JSON line, with the card's name and power limit read in the same run.
 
-    python tools/pass_times.py [--steps K] [--warmup W] [--pass1-blocks 8,6,5]
+    python tools/pass_times.py [--steps K] [--warmup W] [--pass1-blocks 8,6,5] [--ag-narrow rows,duo,rows,duo]
 
 Kernel times come from torch.profiler (CUDA activities) over K steps; the step time from CUDA events over K other steps, with the
-profiler off.  --pass1-blocks runs the steps once per value of SNAPGPU_PASS1_BLOCKS_PER_SM (first-pass CTAs of 8 warps per SM).
+profiler off.  --pass1-blocks runs the steps once per value of SNAPGPU_PASS1_BLOCKS_PER_SM (first-pass CTAs of 8 warps per SM);
+--ag-narrow once per value of SNAPGPU_SINGLE_AG_NARROW (the second pass's narrow-band affine-gap form), in the order given, so that
+repeating the values alternates them.
 Writes nothing; --json PATH also writes the line to PATH.
 """
 from __future__ import annotations
@@ -32,7 +34,7 @@ def card():
         return {"name": None, "error": str(e)}
 
 
-def measure(c, args, batches, pass1_blocks):
+def measure(c, args, batches, pass1_blocks, ag_narrow=""):
     import torch
     from torch.profiler import ProfilerActivity, profile
     from snap_b200 import engine
@@ -41,6 +43,10 @@ def measure(c, args, batches, pass1_blocks):
         os.environ["SNAPGPU_PASS1_BLOCKS_PER_SM"] = str(pass1_blocks)
     else:
         os.environ.pop("SNAPGPU_PASS1_BLOCKS_PER_SM", None)
+    if ag_narrow:
+        os.environ["SNAPGPU_SINGLE_AG_NARROW"] = ag_narrow
+    else:
+        os.environ.pop("SNAPGPU_SINGLE_AG_NARROW", None)
     B = args.batch_reads
     al = engine.SingleAligner(c.idx, engine.default_params(**bench.WORKLOADS["single"]["kw"]), max_batch_reads=B)
     stream = torch.cuda.Stream(c.device)
@@ -79,7 +85,7 @@ def measure(c, args, batches, pass1_blocks):
         d = per.setdefault(key, {"kernel": "sg_align_kernel<%s, %s>" % (m.group(1), m.group(2)), "ms": []})
         d["ms"].append(e.time_range.elapsed_us() / 1e3)
     al.close()
-    out = {"pass1_blocks_per_sm": pass1_blocks or "default", "reads_per_step": B, "deferred_reads_per_step": deferred,
+    out = {"pass1_blocks_per_sm": pass1_blocks or "default", "ag_narrow": ag_narrow or "default", "reads_per_step": B, "deferred_reads_per_step": deferred,
            "step_ms": {"mean": round(sum(step_ms) / len(step_ms), 3), "min": round(min(step_ms), 3), "max": round(max(step_ms), 3)}}
     for key, d in sorted(per.items()):
         ms = d["ms"]
@@ -99,12 +105,14 @@ def main():
     ap.add_argument("--batch-reads", type=int, default=1 << 20)
     ap.add_argument("--batches", type=int, default=3, help="distinct seeded batches the steps cycle through")
     ap.add_argument("--pass1-blocks", default="", help="comma-separated SNAPGPU_PASS1_BLOCKS_PER_SM values to sweep (default: the library's own)")
+    ap.add_argument("--ag-narrow", default="", help="comma-separated SNAPGPU_SINGLE_AG_NARROW values (rows, duo) to run in turn")
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     bargs = argparse.Namespace(genome_mbp=args.genome_mbp, batch_reads=args.batch_reads, repeat_frac=0.0, gpus=1)
     c = bench.build_context(bargs)
     batches = bench.make_batches(c, bargs, "single", args.batches)
-    runs = [measure(c, args, batches, int(v) if v else 0) for v in (args.pass1_blocks.split(",") if args.pass1_blocks else [""])]
+    runs = [measure(c, args, batches, int(v) if v else 0, n) for v in (args.pass1_blocks.split(",") if args.pass1_blocks else [""])
+            for n in (args.ag_narrow.split(",") if args.ag_narrow else [""])]
     line = json.dumps({"workload": bench.WORKLOADS["single"]["cli"], "genome_mbp": args.genome_mbp, "card": card(),
                        "library": os.environ.get("SNAPGPU_LIB") or "snap_b200/csrc/libsnapgpu.so", "runs": runs})
     print(line, flush=True)
