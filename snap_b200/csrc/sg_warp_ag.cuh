@@ -25,137 +25,159 @@ __device__ __forceinline__ int sg_shfl(int v, int src) { return __shfl_sync(0xff
 // lazy-F passes and is written once.  Exactly the nBlocks == 1 case of the general row loop in sg_warp_ag_compute, in a
 // function of its own so that its loop carries no state of the other cases (registers: the kernels run at 64 per thread,
 // and the general function spills inside its loops) and its code is one small contiguous piece.
+//
+// A band of 2w+1 <= segLen columns touches at most two segments in a row, so a row is a first unit and, when the band crosses a
+// segment boundary, a second one that takes the first one's X.  The function is instruction-issue bound (DESIGN.md section 8), so
+// what does not change from unit to unit is a per-lane constant (the offset of a lane's diagonal predecessor, the lazy-F shuffle
+// source), and the kernels' 64 registers decide which ones: values used once per unit are recomputed rather than held.  A unit has
+// no branches but its lazy-F loop: lanes outside the unit load from a cell of the unit (their values are never used) and do not
+// store.
+#ifdef __CUDA_ARCH__
+#define SG_ASSUME_GLOBAL(p) __builtin_assume(__isGlobal(p))      // arena memory: global loads and stores, not generic ones
+#else
+#define SG_ASSUME_GLOBAL(p) ((void)0)
+#endif
 __device__ __noinline__ void sg_warp_ag_rows_banded4(const SgScratch &S, int open, int ext, int dir, const uint8_t *text, int textLen, int patternLen,
                                                      int w, int scoreInit, SgAgLayout &lay, uint8_t *bt, int lane, SgAgBests *res)
 {
+    const int BIG = 1 << 20;             // pushes a term below every F (F and cell values stay below 12000: sg_ag_small_scores)
     const int numVec = lay.numVec, segLen = lay.segLen;
     const int stride = lay.rowStride();
     const int l = lane & 7, q = lane >> 3;
-    int16_t *Hptr = S.agH, *Hm1ptr = S.agHm1, *E = S.agE;
-    const int16_t *prof = S.agProf;
-    int bestG = -1, bestGT = -1, bestL = -1, bestLT = -1, bestLP = -1;
-    const int globalIdx = lay.cellIndex(patternLen - 1);
-    int segBegTrack = 0, segEndTrack = ((w < patternLen - 1) ? w : (patternLen - 1)) / segLen;
+    int16_t *Hptr = S.agH, *Hm1ptr = S.agHm1;
+    int16_t *const E = S.agE;
+    const int16_t *const prof = S.agProf;
+    SG_ASSUME_GLOBAL(Hptr); SG_ASSUME_GLOBAL(Hm1ptr); SG_ASSUME_GLOBAL(E); SG_ASSUME_GLOBAL(prof); SG_ASSUME_GLOBAL(bt);
+    int bestG = -1, bestGT = -1, bestLT = -1;
+    int bestKey = -1;                    // (best local score << 16) | its column, -1 before the first
+    // column patternLen-1 is lane gLane of its segment's unit, and that unit is the last one of every row whose band reaches it
+    const int gLane = lay.cellIndex(patternLen - 1) % segLen;
+
+    // per-lane constants.  Cell of lane (q, l) in the unit of segment j: j*segLen + lane.  Its diagonal predecessor (the previous
+    // row's H one column left): vector q-1 of the same SSE lane, or for q = 0 the segment's last vector in SSE lane l-1, or for
+    // lane 0 the previous segment's last cell (the reference's hInit)
+    const int diagOff = q ? -SG_VEC : (l ? segLen - SG_VEC - 1 : -1);
     const int laneUp = (lane & 24) | ((l + 7) & 7);
+    const int qExt = q * ext;
+
+    int begOff = 0;                                                  // first cell of the row's first segment
+    int endOff = (((w < patternLen - 1) ? w : (patternLen - 1)) / segLen) * segLen;   // ... and of its last
+    // H left of column 0 (the reference's hInit of segment 0): scoreInit in row 0, scoreInit - open - (i-1)*ext after; it only
+    // enters through hdiag > 0 ? .. : 0, so it needs no clamp at 0
+    int rowInit = scoreInit;
+    const uint8_t *tp = text;
+    uint8_t *btRow = bt;
+    int i = 0;
 
     #pragma unroll 1
-    for (int i = 0; i < textLen; i++) {
-        const uint32_t tb = sg_base_value(text[i * dir]);
-        uint8_t *btRow = bt + (size_t)i * stride;
-        const int16_t *profRow = prof + tb * stride;
-        int myMax = 0, myMaxCol = -1, X0 = 0;
+    for (; i < textLen; i++) {
+        const int16_t *profRow = prof + (int)sg_base_value(*tp) * stride;
+        tp += dir;
         const int bandBeg = (i - w) > 0 ? (i - w) : 0;
         const int bandEnd = (i + w) < (patternLen - 1) ? (i + w) : (patternLen - 1);
-        while (bandBeg >= (segBegTrack + 1) * segLen) segBegTrack++;
-        while (bandEnd >= (segEndTrack + 1) * segLen) segEndTrack++;
+        // band edges advance by at most one column per row
+        if (bandBeg >= begOff + segLen) begOff += segLen;
+        if (bandEnd >= endOff + segLen) endOff += segLen;
+        int key = 0;                     // max over my committed cells of (H << 16) | column: the row maximum and its largest column
+        int X0 = 0, h = 0;
 
+        // one unit, or two with the first one's X carried into the second; none once the band has left the last segment
         #pragma unroll 1
-        for (int j = segBegTrack; j <= segEndTrack; j++) {
-            const int vbase = j * numVec;
-            int nVecHere = bandEnd - j * segLen + 1;
-            if (nVecHere > numVec) nVecHere = numVec;
-            if (nVecHere < 0) nVecHere = 0;
-            int hInit;
-            if (j == 0) {
-                hInit = scoreInit;
-                if (i > 0) { hInit = scoreInit - open - (i - 1) * ext; if (hInit < 0) hInit = 0; }
-            } else {
-                hInit = (bandBeg > j * segLen) ? 0 : (int)Hptr[(vbase - 1) * SG_VEC + (SG_VEC - 1)];
-            }
-            const int fcarry = (j > segBegTrack) ? (l == 0 ? X0 : 0) : 0;       // (X0, 0, ..., 0) passed on from the previous segment (:572)
-            const bool valid = q < nVecHere;
-            const int idx = (vbase + q) * SG_VEC + l;
-            int temp = 0, h = 0, act = 0;
-            if (valid) {
-                int hdiag;
-                if (q == 0) hdiag = (l == 0) ? hInit : (int)Hptr[(vbase + numVec - 1) * SG_VEC + l - 1];
-                else hdiag = Hptr[idx - SG_VEC];
-                const int pv = profRow[idx];
-                const int m = (hdiag > 0) ? hdiag + pv : 0;      // (no saturation can occur here: sg_ag_small_scores)
-                const int e = E[idx];
-                act = (e > m) ? 1 : 0;
-                h = m > e ? m : e;
-                const int e2 = e - ext;
-                temp = m - open; if (temp < 0) temp = 0;
-                if (e2 > temp) act |= 4;
-                E[idx] = (int16_t)(e2 > temp ? e2 : temp);
-            }
-            const int t0 = sg_shfl(temp, l), t1 = sg_shfl(temp, 8 + l), t2 = sg_shfl(temp, 16 + l), t3 = sg_shfl(temp, 24 + l);
-            int fin = fcarry - q * ext;
-            if (q > 0) { int v = t0 - (q - 1) * ext; if (v > fin) fin = v; }
-            if (q > 1) { int v = t1 - (q - 2) * ext; if (v > fin) fin = v; }
-            if (q > 2) { int v = t2; if (v > fin) fin = v; }
-            if (valid) {
-                if (fin > h) { act |= 2; h = fin; }
-                if (fin - ext > temp) act |= 32;
-            }
-            int fl = fcarry - nVecHere * ext;            // f register of SSE lane l after the main pass
-            { int v = t0 - (nVecHere - 1) * ext; if (nVecHere > 0 && v > fl) fl = v; }
-            { int v = t1 - (nVecHere - 2) * ext; if (nVecHere > 1 && v > fl) fl = v; }
-            { int v = t2 - (nVecHere - 3) * ext; if (nVecHere > 2 && v > fl) fl = v; }
-            { int v = t3 - (nVecHere - 4) * ext; if (nVecHere > 3 && v > fl) fl = v; }
-            if (fl < 0) fl = 0;
-            // lazy F (:534-569).  Counted on `snap single -d 14`: 4.4 rounds per (row, segment) -- with gap-extend 1
-            // against gap-open 7 the cells right of the diagonal stay within reach of F round after round -- so the round is kept to
-            // the bone: a lane outside the unit holds an H nothing beats (no `valid` tests), "my vector is at or before the first one
-            // with no live lane" is one mask test on the vote, and X (:572) is taken after the loop in closed form -- lane 7 holds SSE
-            // lane 7-r's f, r rounds decayed, at the top of round r -- instead of by a shuffle per round.
-            const unsigned stopBits = 0x80808080u & (nVecHere >= 4 ? 0xffffffffu : ((1u << (8 * nVecHere)) - 1u));
-            const unsigned beforeMe = 0x80808080u & ((1u << (8 * q)) - 1u);
-            const int dRound = nVecHere * ext, fl0 = fl;
-            // 0x3fff beats every F: F is a decayed cell value, and sg_ag_small_scores keeps cell values below 12000 for this form
-            if (!valid) h = 0x3fff;
+        for (int jOff = begOff; jOff <= endOff; jOff += segLen) {
+            const int nv = (bandEnd - jOff + 1) < numVec ? (bandEnd - jOff + 1) : numVec;     // vectors of this segment in the band, >= 1
+            const bool valid = q < nv;
+            const bool ownInit = lane == 0 && (jOff == 0 || bandBeg > jOff);
+            const int hInit = (jOff == 0) ? rowInit : 0;
+            const int cell = jOff + (valid ? lane : 0);
+            const int dcell = (valid && !ownInit) ? cell + diagOff : jOff;
+            const int hd = Hptr[dcell];
+            const int pv = profRow[cell];
+            const int e = E[cell];
+            const int hdiag = ownInit ? hInit : hd;
+            const int m = (hdiag > 0) ? hdiag + pv : 0;      // (no saturation can occur here: sg_ag_small_scores)
+            const int hme = m > e ? m : e;
+            const int e2 = e - ext;
+            int temp = m - open; if (temp < 0) temp = 0;
+            if (valid) E[cell] = (int16_t)(e2 > temp ? e2 : temp);
+            int act = ((e > m) ? 1 : 0) | ((e2 > temp) ? 4 : 0);
+            // F leaving vector q of SSE lane l is max(fcarry - (q+1)*ext, temp[q'] - (q-q')*ext for q' <= q): a prefix max of
+            // temp + q*ext over the 4 vectors (a shuffle up returns a lane's own value where it has no source, which a max absorbs)
+            const int fcarry = (l == 0) ? X0 : 0;          // (X0, 0, ..., 0) passed on from the previous segment (:572)
+            int s = temp + qExt;
+            { const int v = __shfl_up_sync(0xffffffffu, s, 8); if (v > s) s = v; }
+            { const int v = __shfl_up_sync(0xffffffffu, s, 16); if (v > s) s = v; }
+            const int fout = ((fcarry - ext) > s ? (fcarry - ext) : s) - qExt;
+            const int fup = __shfl_up_sync(0xffffffffu, fout, 8);
+            const int fin = q ? fup : fcarry;              // F entering my vector
+            h = hme > fin ? hme : fin;
+            if (fin - ext > temp) act |= 32;
+            // f register of SSE lane l after the main pass: F leaving the unit's last vector
+            const int fl0 = sg_shfl(fout, ((nv - 1) << 3) | l);
+            // lazy F (:534-569).  Counted on `snap single -d 14`: 4.4 rounds per (row, segment) -- with gap-extend 1 against
+            // gap-open 7 the cells right of the diagonal stay within reach of F round after round -- so the round is kept to the
+            // bone.  f carries -q*ext and is never clamped at 0: every use of it (max with H >= 0, f > H, f - ext > max(.., 0))
+            // gives the same answer for a negative f as for 0.  Lane 7 carries BIG less, so that SSE lane 0 takes a value below 0.
+            // A lane outside the unit votes in a byte the stop mask ignores.  Every round but the last commits in every lane; the
+            // last commits up to the first vector with no live lane.  H rises only where F beat it, so bit 2 is read off H.
+            const unsigned stopBits = 0x80808080u >> (32 - 8 * nv);
+            const int dRound = nv * ext, dec = dRound + ((l == 7) ? BIG : 0);
+            int f = fl0 - qExt - ((l == 7) ? BIG : 0);
             int nRounds = 0;
+            bool liveAny = false;
             #pragma unroll 1
-            for (int kk = 0; kk < SG_VEC - 1; kk++) {
+            for (;;) {
+                f = sg_shfl(f, laneUp);
                 nRounds++;
-                { const int up = sg_shfl(fl, laneUp); fl = (l == 0) ? 0 : up; }
-                int fv = fl - q * ext; if (fv < 0) fv = 0;
-                const int newh = fv > h ? fv : h;
+                const int newh = f > h ? f : h;
                 int tmp2 = newh - open; if (tmp2 < 0) tmp2 = 0;
-                int fn = fv - ext; if (fn < 0) fn = 0;
-                const bool live = fn > tmp2;
+                const bool live = f - ext > tmp2;
                 const unsigned liveMask = __ballot_sync(0xffffffffu, live);
                 // lowest all-zero byte of the ballot among the unit's vectors = first vector at which no lane is live
                 const unsigned zb = (liveMask - 0x01010101u) & ~liveMask & stopBits;
-                if (!(zb & beforeMe)) {
-                    if (fv > h) act |= 2;
-                    if (live) act |= 32;
-                    h = newh;
+                if (zb) {
+                    const unsigned beforeMe = 0x80808080u & ((1u << (lane & 24)) - 1u);     // the bytes of the vectors before mine
+                    if (!(zb & beforeMe)) { h = newh; liveAny |= live; }
+                    break;
                 }
-                if (zb) break;
-                fl = fl - dRound; if (fl < 0) fl = 0;
+                h = newh; liveAny |= live;
+                if (nRounds == SG_VEC - 1) break;
+                f -= dec;
             }
-            if (j < segEndTrack) {        // X only feeds the next segment of this row
+            if (h > hme) act |= 2;
+            if (liveAny) act |= 32;
+            if (valid) {
+                Hm1ptr[cell] = (int16_t)h;
+                btRow[cell] = (uint8_t)act;
+                const int k = (h << 16) | (jOff + l * numVec + q);     // (a lane's columns rise from unit to unit: ties go to the later)
+                if (k > key) key = k;
+            }
+            if (jOff < endOff) {
+                // X (:572) only feeds the next segment of this row, in closed form: lane 7 holds SSE lane 7-r's f, r rounds
+                // decayed, at the top of round r
                 int v = fl0 - (7 - l) * dRound;
                 if (v < 0 || (7 - l) >= nRounds) v = 0;
-                v = __reduce_max_sync(0xffffffffu, v);
-                if (v > X0) X0 = v;
+                X0 = __reduce_max_sync(0xffffffffu, v);
             }
-            if (valid) {
-                const int col = j * segLen + l * numVec + q;
-                if (h > myMax || (h == myMax && col > myMaxCol)) { myMax = h; myMaxCol = col; }
-                Hm1ptr[idx] = (int16_t)h;
-                btRow[idx] = (uint8_t)act;
-            }
-            __syncwarp();
         }
+        __syncwarp();
 
-        const int maxScoreRow = __reduce_max_sync(0xffffffffu, myMax);
+        const int rowKey = __reduce_max_sync(0xffffffffu, key);
         if (bandEnd == patternLen - 1) {
-            const int globalAlignmentScore = Hm1ptr[globalIdx];
+            // the last unit holds the cell in lane gLane; with no unit in the row, the reference reads the row two rows back
+            const int globalAlignmentScore = (begOff <= endOff) ? sg_shfl(h, gLane) : (int)Hm1ptr[endOff + gLane];
             if (globalAlignmentScore >= bestG) { bestG = globalAlignmentScore; bestGT = i; }
         }
-        lay.nRows = i + 1;
+        const int maxScoreRow = rowKey >> 16;
         if (maxScoreRow == 0) break;
-        if (maxScoreRow > bestL) {
-            bestL = maxScoreRow; bestLT = i;
-            bestLP = __reduce_max_sync(0xffffffffu, (myMax == maxScoreRow) ? myMaxCol : -1);
-        }
+        if (maxScoreRow > (bestKey >> 16)) { bestKey = rowKey; bestLT = i; }
         int16_t *tmp = Hm1ptr; Hm1ptr = Hptr; Hptr = tmp;
+        btRow += stride;
+        rowInit -= (i == 0) ? open : ext;
     }
+    lay.nRows = (i < textLen) ? i + 1 : i;
     __syncwarp();
-    res->gScore = bestG; res->gText = bestGT; res->lScore = bestL; res->lText = bestLT; res->lPat = bestLP;
+    res->gScore = bestG; res->gText = bestGT; res->lScore = bestKey < 0 ? -1 : bestKey >> 16; res->lText = bestLT;
+    res->lPat = bestKey < 0 ? -1 : bestKey & 0xffff;
 }
 
 
