@@ -22,11 +22,12 @@
 extern "C" {
 #endif
 
-#define SNAPGPU_ABI_VERSION 8   /* 2: snapgpu_sam_format_* take frontClipped / clippedLens before `results`; 3: groups, replicate, host_alloc, random-sector rate;
+#define SNAPGPU_ABI_VERSION 9   /* 2: snapgpu_sam_format_* take frontClipped / clippedLens before `results`; 3: groups, replicate, host_alloc, random-sector rate;
                                  * 4: snapgpu_sam_sort_device; 5: snapgpu_bam_markdup_device, snapgpu_bam_index_device;
                                  * 6: snapgpu_align_single_secondary(_device) (-om), snapgpu_bgzf_deflate_device, snapgpu_bam_index_members_device, snapgpu_sam_header;
                                  * 7: snapgpu_contig, snapgpu_index_build_genome(_device), snapgpu_save_options, snapgpu_index_save_ex;
-                                 * 8: snapgpu_aligner_deferred_count */
+                                 * 8: snapgpu_aligner_deferred_count;
+                                 * 9: snapgpu_spacing_* and snapgpu_align_paired_ins(_device) (`snap paired -ins`) */
 
 /* AlignmentResult enum, reference SNAPLib/AlignmentResult.h:34 */
 enum { SNAPGPU_NOT_FOUND = 0, SNAPGPU_SINGLE_HIT = 1, SNAPGPU_MULTIPLE_HITS = 2 };
@@ -393,6 +394,39 @@ int  snapgpu_align_paired_device(snapgpu_aligner *a, int64_t nPairs, const char 
                                  const uint64_t *d_offsets, const uint32_t *d_lens,
                                  snapgpu_paired_result *d_results, snapgpu_counters *d_counters,
                                  void *cudaStream);
+
+/*
+ * Insert-size inference (`snap paired -ins`, reference PairedAligner.cpp:889-925).  An estimator holds what stock keeps per worker
+ * thread: a window of samples and the current (minSpacing, maxSpacing).  A pair that is not useless adds a sample when its
+ * primary record passes the filters (`filterFlags`, after the -fs fix-up) and its ends are FORWARD/RC or RC/FORWARD: the distance
+ * between the two locations.  When the window holds `window` samples it is sorted and the new range computed
+ * (PairedAligner.cpp:424-458); the pair after the one that filled it is the first aligned with that range.
+ *
+ * snapgpu_spacing_create: the initial range is the aligner's -s range.  filterFlags takes the bits of AlignerOptions::filterFlags
+ * (FilterUnaligned 0x1, FilterSingleHit 0x2, FilterMultipleHits 0x4, FilterBothMatesMatch 0x8, FilterTooShort 0x10; -F a is 0x16).  window 0 means 262144, stock's; any other value (4..262144) is a test
+ * seam only and does not reproduce stock.  The estimator lives on the aligner's device and may be used with any paired aligner
+ * handle on that device.
+ */
+typedef struct snapgpu_spacing snapgpu_spacing;
+int  snapgpu_spacing_create(const snapgpu_aligner *a, int32_t filterFlags, int64_t window, snapgpu_spacing **out);
+void snapgpu_spacing_destroy(snapgpu_spacing *est);
+/* The current range, the samples taken so far and the number of range updates. */
+int  snapgpu_spacing_get(const snapgpu_spacing *est, int32_t *minSpacing, uint32_t *maxSpacing, int64_t *samples, int64_t *updates);
+/* Alignment sub-launches issued for this estimator, and the host seconds spent sorting full windows and computing their ranges. */
+int  snapgpu_spacing_timing(const snapgpu_spacing *est, int64_t *subLaunches, double *statSeconds);
+
+/* snapgpu_align_paired under insert-size inference: every pair is aligned with the range stock would use for it, and the
+ * estimator's state carries over between calls, so results do not depend on how the pairs are split into calls.  The pairs run in
+ * sub-launches; a call makes at most 5 per range update it performs, plus 5.  Counters count each pair once.  A kernel error
+ * (see snapgpu_aligner_check) fails the call and leaves the estimator as it was before the sub-launch that raised it. */
+int  snapgpu_align_paired_ins(snapgpu_aligner *a, snapgpu_spacing *est, int64_t nPairs, const char *bases, const char *quals,
+                              const uint64_t *offsets, const uint32_t *lens,
+                              snapgpu_paired_result *results, snapgpu_counters *counters);
+/* Device-pointer form.  Not asynchronous: it synchronises `cudaStream` (NULL = the aligner's own) after every sub-launch to read the
+ * sample count back.  d_counters (may be NULL) are added to, as snapgpu_align_paired_device does. */
+int  snapgpu_align_paired_ins_device(snapgpu_aligner *a, snapgpu_spacing *est, int64_t nPairs, const char *d_bases, const char *d_quals,
+                                     const uint64_t *d_offsets, const uint32_t *d_lens,
+                                     snapgpu_paired_result *d_results, snapgpu_counters *d_counters, void *cudaStream);
 
 /* Synchronises `cudaStream` (NULL = the aligner's own) and returns non-zero (message in snapgpu_last_error) if a
  * kernel of this aligner latched an error since the last check. */

@@ -21,7 +21,10 @@
  *   single: SingleAligner.cpp:197-338 (pre-filter :213, AlignRead :250, passFilter + writeReads :296-322, updateStats :354-374)
  *   paired: PairedAligner.cpp:654-927 (id check :664, useful0/1 :676-678, align :727, forceSpacing :822, passFilter :832-850,
  *           writePairs :870, updateStats :962-1010)
- * Not supported (fails loudly, never falls back to the CPU aligner): secondary alignments (-om) of `paired`, 64-bit indexes, -ins.
+ * `paired -ins` (insert-size inference, PairedAligner.cpp:889-925) keeps its state per worker thread as stock does: each thread has
+ * its own estimator (snapgpu_spacing) on its device and aligns its batches with snapgpu_align_paired_ins, so `-t 1` writes what
+ * stock `-t 1` writes.  As in stock, with -t N the result depends on which pairs each thread reads.
+ * Not supported (fails loudly, never falls back to the CPU aligner): secondary alignments (-om) of `paired`, 64-bit indexes.
  */
 #include "stdafx.h"
 #include "Compat.h"
@@ -353,10 +356,6 @@ GpuEngine *GpuAlignerExtension::engineForThisThread(AlignerContext *context, boo
             pp.enableHammingScoringBaseAligner = po->enableHammingScoringBaseAligner ? 1 : 0;
             pp.useSoftClipping = context->options->useSoftClipping ? 1 : 0;
             pp.flattenMAPQAtOrBelow = context->options->flattenMAPQAtOrBelow;
-            if (po->inferSpacing) {
-                WriteErrorMessage("snap-aligner-gpu: -ins (insert size inference makes results depend on the thread partition) is not supported\n");
-                soft_exit(1);
-            }
             if (snapgpu_paired_aligner_create(e->index, &p, &pp, shared->batchReads / 2, &e->aligner)) gpuFatal("creating the paired-end aligner");
         }
     }
@@ -530,6 +529,13 @@ bool GpuAlignerExtension::runIterationThread(PairedReadSupplier *supplier, Align
     snapgpu_counters counters;
     memset(&counters, 0, sizeof(counters));
     const int maxDist = (int)context->maxDist;
+    snapgpu_spacing *spacing = NULL;         // -ins: this thread's window (stock keeps it per thread, in PairedAlignerContext)
+    if (po->inferSpacing) {
+        pthread_mutex_lock(&engine->lock);
+        const int rc = snapgpu_spacing_create(engine->aligner, options->filterFlags, 0, &spacing);
+        pthread_mutex_unlock(&engine->lock);
+        if (rc) gpuFatal("snapgpu_spacing_create");
+    }
 
     Read *reads[NUM_READS_PER_PAIR] = {NULL, NULL};
     bool more = supplier->getNextReadPair(&reads[0], &reads[1]);
@@ -544,9 +550,10 @@ bool GpuAlignerExtension::runIterationThread(PairedReadSupplier *supplier, Align
         }
         const _int64 nPairs = batch.n / 2;
         pthread_mutex_lock(&engine->lock);
-        const int rc = snapgpu_align_paired(engine->aligner, nPairs, batch.bases, batch.quals, batch.offsets, batch.lens, results, &counters);
+        const int rc = spacing ? snapgpu_align_paired_ins(engine->aligner, spacing, nPairs, batch.bases, batch.quals, batch.offsets, batch.lens, results, &counters)
+                               : snapgpu_align_paired(engine->aligner, nPairs, batch.bases, batch.quals, batch.offsets, batch.lens, results, &counters);
         pthread_mutex_unlock(&engine->lock);
-        if (rc) gpuFatal("snapgpu_align_paired");
+        if (rc) gpuFatal(spacing ? "snapgpu_align_paired_ins" : "snapgpu_align_paired");
 
         for (_int64 i = 0; i < nPairs; i++) {
             Read *pr[NUM_READS_PER_PAIR] = {&batch.reads[2 * i], &batch.reads[2 * i + 1]};
@@ -617,6 +624,11 @@ bool GpuAlignerExtension::runIterationThread(PairedReadSupplier *supplier, Align
     stats->lvCalls = counters.lvCalls;
     stats->affineGapCalls = counters.affineGapCalls;
     addCounters(engine, counters);
+    if (spacing) {
+        pthread_mutex_lock(&engine->lock);
+        snapgpu_spacing_destroy(spacing);
+        pthread_mutex_unlock(&engine->lock);
+    }
     batch.destroy();
     snapgpu_host_free(results);
     return true;

@@ -14,6 +14,7 @@
 #include <sys/types.h>
 #include <string>
 #include <vector>
+#include <chrono>
 #include <algorithm>
 #include <functional>
 #include <new>
@@ -29,6 +30,7 @@
 #include "sg_bampost.h"
 #include "sg_deflate.h"
 #include "sg_samheader.h"
+#include "sg_spacing.h"
 
 // ------------------------------------------------------------------------------------------------
 // error plumbing
@@ -2585,6 +2587,377 @@ int snapgpu_align_paired(snapgpu_aligner *a, int64_t nPairs, const char *bases, 
     if (nPairs < 0 || 2 * nPairs > a->maxBatchReads) return sg_fail("pair count exceeds maxBatchPairs");
     if (nPairs == 0) return 0;
     return align_host(a, nPairs, 2, sizeof(snapgpu_paired_result), bases, quals, offsets, lens, (uint8_t *)results, counters);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Insert-size inference (`snap paired -ins`, sg_spacing.h)
+//
+// A call aligns its pairs in sub-launches and keeps every pair under the range stock would use for it.  A pair adds at most one
+// sample, so a sub-launch of at most d = W - count pairs cannot hold a cut before its last pair ("safe").  A longer one is
+// speculative: if the window fills at pair j before its end, the launch's counters are put back, [p, j] is aligned again under
+// the same range (for its counters; the records are the same), and the pairs after j go on under the new range.
+// Per window update a call makes: two safe sub-launches, then a speculative one of about twice the pairs the window's sample rate
+// says are needed, then one of all the pairs left, then the realignment: SG_SPACING_LAUNCHES_PER_UPDATE in all.
+// ------------------------------------------------------------------------------------------------
+#define SG_SPACING_LAUNCHES_PER_UPDATE 5
+
+static double sg_now_seconds()
+{
+    return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
+}
+
+struct snapgpu_spacing {
+    int device = 0;
+    int32_t filterFlags = 0;
+    int32_t forceSpacing = 0;
+    int64_t window = SG_SPACING_WINDOW;
+    int32_t minSpacing = 0;
+    uint32_t maxSpacing = 0;
+    int64_t count = 0, samples = 0, updates = 0;
+    int64_t windowPairs = 0, windowSamples = 0;      // pairs aligned and samples taken since the last update: the sample rate
+    int64_t subLaunches = 0;
+    double statSeconds = 0;
+    int64_t *d_window = nullptr, *d_sorted = nullptr, *h_sorted = nullptr;
+    void *d_sortTemp = nullptr; size_t sortTempBytes = 0;
+    // per-pair scratch of one sub-launch, grown on demand
+    int64_t pairCap = 0;
+    int64_t *d_dist = nullptr; int32_t *d_flag = nullptr, *d_pos = nullptr;
+    void *d_scanTemp = nullptr; size_t scanTempBytes = 0;
+    int64_t *d_io = nullptr, *h_io = nullptr;         // [0] inclusive sample count of the sub-launch, [1] the pair that fills the window,
+                                                      // [2] the aligner's latched error code
+    snapgpu_counters *d_ctrSave = nullptr, *d_ctr = nullptr, *h_ctr = nullptr;
+    // staging of the host-buffer entry, grown on demand
+    int64_t stagePairs = 0; size_t stageBases = 0;
+    char *d_bases = nullptr, *d_quals = nullptr; uint64_t *d_offsets = nullptr; uint32_t *d_lens = nullptr;
+    snapgpu_paired_result *d_results = nullptr;
+};
+
+__global__ void __launch_bounds__(256) sg_spacing_sample_kernel(int64_t n, const snapgpu_paired_result *results, const uint8_t *bases,
+                                                                const unsigned long long *offsets, const uint32_t *lens, uint32_t minReadLength,
+                                                                int maxK, uint32_t maxReadLen, int32_t filterFlags, int32_t forceSpacing,
+                                                                int64_t *dist, int32_t *flag)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    bool useful[2], tooLong = false;
+    for (int w = 0; w < 2; w++) {
+        const uint8_t *b = bases + offsets[2 * i + w];
+        const uint32_t len = lens[2 * i + w];
+        int countOfNs = 0;
+        for (uint32_t k = 0; k < len; k++) countOfNs += b[k] == 'N';
+        useful[w] = len >= minReadLength && countOfNs <= maxK;         // as the paired kernel decides it
+        tooLong = tooLong || len > maxReadLen;
+    }
+    if (tooLong) useful[0] = useful[1] = false;
+    const int64_t s = sg_spacing_sample(results[i], useful, filterFlags, forceSpacing != 0, SNAPGPU_INVALID_LOCATION_32);
+    dist[i] = s;
+    flag[i] = s >= 0;
+}
+
+// Appends the sub-launch's samples in pair order at `count`; io[1] = the pair whose sample fills the window.
+__global__ void __launch_bounds__(256) sg_spacing_append_kernel(int64_t n, const int64_t *dist, const int32_t *pos, int64_t count, int64_t window,
+                                                                int64_t *out, int64_t *io)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (i == n - 1) io[0] = pos[i];
+    if (dist[i] < 0) return;
+    const int64_t k = count + pos[i] - 1;
+    if (k < window) out[k] = dist[i];
+    if (k == window - 1) io[1] = i;
+}
+
+static void spacing_free(snapgpu_spacing *e)
+{
+    cudaFree(e->d_window); cudaFree(e->d_sorted); cudaFreeHost(e->h_sorted); cudaFree(e->d_sortTemp);
+    cudaFree(e->d_dist); cudaFree(e->d_flag); cudaFree(e->d_pos); cudaFree(e->d_scanTemp);
+    cudaFree(e->d_io); cudaFreeHost(e->h_io); cudaFree(e->d_ctrSave); cudaFree(e->d_ctr); cudaFreeHost(e->h_ctr);
+    cudaFree(e->d_bases); cudaFree(e->d_quals); cudaFree(e->d_offsets); cudaFree(e->d_lens); cudaFree(e->d_results);
+}
+
+int snapgpu_spacing_create(const snapgpu_aligner *a, int32_t filterFlags, int64_t window, snapgpu_spacing **out)
+{
+    if (!a || !out) return sg_fail("null argument");
+    *out = nullptr;
+    if (!a->paired) return sg_fail("snapgpu_spacing_create: the aligner is not a paired-end one");
+    if (window < 0 || window > SG_SPACING_WINDOW) return sg_fail("snapgpu_spacing_create: window must be 0 (262144) or 4..262144");
+    if (window == 0) window = SG_SPACING_WINDOW;
+    if (window < 4) return sg_fail("snapgpu_spacing_create: window must be 0 (262144) or 4..262144");
+    SG_CUDA(cudaSetDevice(a->device));
+    snapgpu_spacing *e = new snapgpu_spacing();
+    e->device = a->device;
+    e->filterFlags = filterFlags;
+    e->forceSpacing = a->pparams.forceSpacing;
+    e->window = window;
+    e->minSpacing = a->pparams.minSpacing;
+    e->maxSpacing = a->pparams.maxSpacing;
+    cudaError_t err = cudaMalloc((void **)&e->d_window, (size_t)window * 8);
+    if (err == cudaSuccess) err = cudaMalloc((void **)&e->d_sorted, (size_t)window * 8);
+    if (err == cudaSuccess) err = cudaMallocHost((void **)&e->h_sorted, (size_t)window * 8);
+    if (err == cudaSuccess) err = cudaMalloc((void **)&e->d_io, 24);
+    if (err == cudaSuccess) err = cudaMallocHost((void **)&e->h_io, 24);
+    if (err == cudaSuccess) err = cudaMalloc((void **)&e->d_ctrSave, sizeof(snapgpu_counters));
+    if (err == cudaSuccess) err = cudaMalloc((void **)&e->d_ctr, sizeof(snapgpu_counters));
+    if (err == cudaSuccess) err = cudaMallocHost((void **)&e->h_ctr, sizeof(snapgpu_counters));
+    if (err == cudaSuccess) err = cub::DeviceRadixSort::SortKeys(nullptr, e->sortTempBytes, e->d_window, e->d_sorted, (int)window);
+    if (err == cudaSuccess) err = cudaMalloc(&e->d_sortTemp, e->sortTempBytes);
+    if (err != cudaSuccess) {
+        spacing_free(e); delete e;
+        return sg_fail(std::string("snapgpu_spacing_create: ") + cudaGetErrorString(err));
+    }
+    *out = e;
+    return 0;
+}
+
+void snapgpu_spacing_destroy(snapgpu_spacing *e)
+{
+    if (!e) return;
+    cudaSetDevice(e->device);
+    spacing_free(e);
+    delete e;
+}
+
+int snapgpu_spacing_get(const snapgpu_spacing *e, int32_t *minSpacing, uint32_t *maxSpacing, int64_t *samples, int64_t *updates)
+{
+    if (!e) return sg_fail("null argument");
+    if (minSpacing) *minSpacing = e->minSpacing;
+    if (maxSpacing) *maxSpacing = e->maxSpacing;
+    if (samples) *samples = e->samples;
+    if (updates) *updates = e->updates;
+    return 0;
+}
+
+int snapgpu_spacing_timing(const snapgpu_spacing *e, int64_t *subLaunches, double *statSeconds)
+{
+    if (!e) return sg_fail("null argument");
+    if (subLaunches) *subLaunches = e->subLaunches;
+    if (statSeconds) *statSeconds = e->statSeconds;
+    return 0;
+}
+
+static int spacing_reserve(snapgpu_spacing *e, int64_t nPairs)
+{
+    if (nPairs <= e->pairCap) return 0;
+    cudaFree(e->d_dist); cudaFree(e->d_flag); cudaFree(e->d_pos); cudaFree(e->d_scanTemp);
+    e->d_dist = nullptr; e->d_flag = e->d_pos = nullptr; e->d_scanTemp = nullptr; e->pairCap = 0;
+    SG_CUDA(cudaMalloc((void **)&e->d_dist, (size_t)nPairs * 8));
+    SG_CUDA(cudaMalloc((void **)&e->d_flag, (size_t)nPairs * 4));
+    SG_CUDA(cudaMalloc((void **)&e->d_pos, (size_t)nPairs * 4));
+    SG_CUDA(cub::DeviceScan::InclusiveSum(nullptr, e->scanTempBytes, e->d_flag, e->d_pos, (int)nPairs));
+    SG_CUDA(cudaMalloc(&e->d_scanTemp, e->scanTempBytes));
+    e->pairCap = nPairs;
+    return 0;
+}
+
+// The window is full: sort it on the device, and compute the range on the host from the sorted copy.  The two sums must run in
+// sorted order to give stock's bits, so on the device they would be one thread's chain of 2 x 262144 dependent double adds; the
+// host was chosen on that reasoning, not on a timing of both (see DESIGN §3).  statSeconds times this whole function.
+static int spacing_update(snapgpu_spacing *e, cudaStream_t st)
+{
+    const double t0 = sg_now_seconds();
+    SG_CUDA(cub::DeviceRadixSort::SortKeys(e->d_sortTemp, e->sortTempBytes, e->d_window, e->d_sorted, (int)e->window, 0, 64, st));
+    SG_CUDA(cudaMemcpyAsync(e->h_sorted, e->d_sorted, (size_t)e->window * 8, cudaMemcpyDeviceToHost, st));
+    SG_CUDA(cudaStreamSynchronize(st));
+    int32_t mn = 0, mx = 0;
+    sg_spacing_range(e->h_sorted, e->window, &mn, &mx);
+    e->minSpacing = mn;
+    e->maxSpacing = (uint32_t)mx;            // IntersectingPairedEndAligner::setMaxSpacing(int) into an unsigned
+    e->count = 0; e->windowPairs = 0; e->windowSamples = 0;
+    e->updates++;
+    e->statSeconds += sg_now_seconds() - t0;
+    return 0;
+}
+
+static int align_paired_ins_impl(snapgpu_aligner *a, snapgpu_spacing *e, int64_t n, const char *d_bases, const char *d_quals,
+                                 const uint64_t *d_offsets, const uint32_t *d_lens, snapgpu_paired_result *d_results,
+                                 snapgpu_counters *d_counters, cudaStream_t st)
+{
+    if (spacing_reserve(e, n)) return 1;
+    int64_t p = 0;
+    int k = 0;                       // sub-launches since the last update in this call
+    while (p < n) {
+        const int64_t rem = n - p, d = e->window - e->count;
+        int64_t c;
+        if (k < 2 || rem <= d) c = std::min(rem, d);
+        else if (k == 2 && e->windowSamples > 0) c = std::min(rem, std::max(d, (2 * d * e->windowPairs + e->windowSamples - 1) / e->windowSamples));
+        else c = rem;
+        const bool speculative = c > d;
+        if (speculative && d_counters) SG_CUDA(cudaMemcpyAsync(e->d_ctrSave, d_counters, sizeof(snapgpu_counters), cudaMemcpyDeviceToDevice, st));
+        a->pparams.minSpacing = a->pparamsBig.minSpacing = e->minSpacing;
+        a->pparams.maxSpacing = a->pparamsBig.maxSpacing = e->maxSpacing;
+        if (launch_align(a, c, d_bases, d_quals, d_offsets + 2 * p, d_lens + 2 * p, d_results + p, d_counters, st)) return 1;
+        e->subLaunches++; k++;
+        const int blocks = (int)((c + 255) / 256);
+        sg_spacing_sample_kernel<<<blocks, 256, 0, st>>>(c, d_results + p, (const uint8_t *)d_bases, (const unsigned long long *)(d_offsets + 2 * p),
+                                                         d_lens + 2 * p, a->params.minReadLength, (int)a->params.maxK, a->params.maxReadLen, e->filterFlags,
+                                                         e->forceSpacing, e->d_dist, e->d_flag);
+        SG_CUDA(cudaGetLastError());
+        SG_CUDA(cub::DeviceScan::InclusiveSum(e->d_scanTemp, e->scanTempBytes, e->d_flag, e->d_pos, (int)c, st));
+        SG_CUDA(cudaMemsetAsync(e->d_io + 1, 0xff, 8, st));
+        sg_spacing_append_kernel<<<blocks, 256, 0, st>>>(c, e->d_dist, e->d_pos, e->count, e->window, e->d_window, e->d_io);
+        SG_CUDA(cudaGetLastError());
+        SG_CUDA(cudaMemcpyAsync(e->h_io, e->d_io, 16, cudaMemcpyDeviceToHost, st));
+        e->h_io[2] = 0;
+        SG_CUDA(cudaMemcpyAsync(&e->h_io[2], a->d_error, sizeof(int), cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaStreamSynchronize(st));
+        // a kernel error (an over-long read, an overflowed pool) leaves the estimator as it was before this sub-launch
+        if (e->h_io[2] != 0) return snapgpu_aligner_check(a, st) ? 1 : sg_fail("aligner kernel reported an error");
+        const int64_t cut = e->h_io[1];
+        if (cut >= 0 && cut < c - 1) {
+            // the window filled inside a speculative sub-launch: only [p, cut] belongs to the old range
+            c = cut + 1;
+            if (d_counters) {
+                SG_CUDA(cudaMemcpyAsync(d_counters, e->d_ctrSave, sizeof(snapgpu_counters), cudaMemcpyDeviceToDevice, st));
+                if (launch_align(a, c, d_bases, d_quals, d_offsets + 2 * p, d_lens + 2 * p, d_results + p, d_counters, st)) return 1;
+                e->subLaunches++;
+            }
+        }
+        const int64_t taken = std::min(e->h_io[0], d);
+        e->count += taken; e->samples += taken;
+        e->windowPairs += c; e->windowSamples += taken;
+        p += c;
+        if (e->count == e->window) {
+            if (spacing_update(e, st)) return 1;
+            k = 0;
+        }
+    }
+    return 0;
+}
+
+// The handle is shared (the drop-in has one per device and one estimator per worker thread): its own range is put back after
+// every call.
+static int align_paired_ins(snapgpu_aligner *a, snapgpu_spacing *e, int64_t n, const char *d_bases, const char *d_quals,
+                            const uint64_t *d_offsets, const uint32_t *d_lens, snapgpu_paired_result *d_results,
+                            snapgpu_counters *d_counters, cudaStream_t st)
+{
+    const int32_t min0 = a->pparams.minSpacing, minBig0 = a->pparamsBig.minSpacing;
+    const uint32_t max0 = a->pparams.maxSpacing, maxBig0 = a->pparamsBig.maxSpacing;
+    const int rc = align_paired_ins_impl(a, e, n, d_bases, d_quals, d_offsets, d_lens, d_results, d_counters, st);
+    a->pparams.minSpacing = min0; a->pparamsBig.minSpacing = minBig0;
+    a->pparams.maxSpacing = max0; a->pparamsBig.maxSpacing = maxBig0;
+    return rc;
+}
+
+static int spacing_check(snapgpu_aligner *a, snapgpu_spacing *e, int64_t nPairs)
+{
+    if (!a->paired) return sg_fail("snapgpu_align_paired_ins called on a single-end aligner handle");
+    if (e->device != a->device) return sg_fail("snapgpu_align_paired_ins: the estimator was created for another device");
+    if (nPairs < 0 || 2 * nPairs > a->maxBatchReads) return sg_fail("pair count exceeds maxBatchPairs");
+    return 0;
+}
+
+int snapgpu_align_paired_ins_device(snapgpu_aligner *a, snapgpu_spacing *e, int64_t nPairs, const char *d_bases, const char *d_quals,
+                                    const uint64_t *d_offsets, const uint32_t *d_lens, snapgpu_paired_result *d_results,
+                                    snapgpu_counters *d_counters, void *cudaStream)
+{
+    if (!a || !e || !d_bases || !d_quals || !d_offsets || !d_lens || !d_results) return sg_fail("null argument");
+    if (spacing_check(a, e, nPairs)) return 1;
+    if (nPairs == 0) return 0;
+    SG_CUDA(cudaSetDevice(a->device));
+    cudaStream_t st = cudaStream ? (cudaStream_t)cudaStream : a->stream;
+    return align_paired_ins(a, e, nPairs, d_bases, d_quals, d_offsets, d_lens, d_results, d_counters, st);
+}
+
+// A host-buffer call that cannot hold a cut before its last pair (nPairs <= W - count; the drop-in's batches, mostly): the pipelined
+// host path of snapgpu_align_paired under the estimator's range, then the samples from the host copies of the results and reads.
+static int align_paired_ins_one_launch(snapgpu_aligner *a, snapgpu_spacing *e, int64_t nPairs, const char *bases, const char *quals,
+                                       const uint64_t *offsets, const uint32_t *lens, snapgpu_paired_result *results, snapgpu_counters *counters)
+{
+    const int32_t min0 = a->pparams.minSpacing, minBig0 = a->pparamsBig.minSpacing;
+    const uint32_t max0 = a->pparams.maxSpacing, maxBig0 = a->pparamsBig.maxSpacing;
+    a->pparams.minSpacing = a->pparamsBig.minSpacing = e->minSpacing;
+    a->pparams.maxSpacing = a->pparamsBig.maxSpacing = e->maxSpacing;
+    const int rc = align_host(a, nPairs, 2, sizeof(snapgpu_paired_result), bases, quals, offsets, lens, (uint8_t *)results, counters);
+    a->pparams.minSpacing = min0; a->pparamsBig.minSpacing = minBig0;
+    a->pparams.maxSpacing = max0; a->pparamsBig.maxSpacing = maxBig0;
+    if (rc) return 1;
+    e->subLaunches++;
+    int64_t taken = 0;
+    for (int64_t i = 0; i < nPairs; i++) {
+        bool useful[2], tooLong = false;
+        for (int w = 0; w < 2; w++) {       // as sg_spacing_sample_kernel decides it
+            const char *b = bases + offsets[2 * i + w];
+            const uint32_t len = lens[2 * i + w];
+            uint32_t countOfNs = 0;
+            for (uint32_t k = 0; k < len; k++) countOfNs += b[k] == 'N';
+            useful[w] = len >= a->params.minReadLength && countOfNs <= a->params.maxK;
+            tooLong = tooLong || len > a->params.maxReadLen;
+        }
+        if (tooLong) useful[0] = useful[1] = false;
+        const int64_t smp = sg_spacing_sample(results[i], useful, e->filterFlags, e->forceSpacing != 0, SNAPGPU_INVALID_LOCATION_32);
+        if (smp >= 0) e->h_sorted[taken++] = smp;        // staging only: h_sorted is rewritten by the next update
+    }
+    if (taken) SG_CUDA(cudaMemcpy(e->d_window + e->count, e->h_sorted, (size_t)taken * 8, cudaMemcpyHostToDevice));
+    e->count += taken; e->samples += taken;
+    e->windowPairs += nPairs; e->windowSamples += taken;
+    if (e->count == e->window && spacing_update(e, a->stream)) return 1;
+    return 0;
+}
+
+int snapgpu_align_paired_ins(snapgpu_aligner *a, snapgpu_spacing *e, int64_t nPairs, const char *bases, const char *quals,
+                             const uint64_t *offsets, const uint32_t *lens, snapgpu_paired_result *results, snapgpu_counters *counters)
+{
+    if (!a || !e || !bases || !quals || !offsets || !lens || !results) return sg_fail("null argument");
+    if (spacing_check(a, e, nPairs)) return 1;
+    if (nPairs == 0) return 0;
+    SG_CUDA(cudaSetDevice(a->device));
+    if (nPairs <= e->window - e->count) return align_paired_ins_one_launch(a, e, nPairs, bases, quals, offsets, lens, results, counters);
+    // pack the reads back to back, as the device entry takes them
+    std::vector<uint64_t> off((size_t)(2 * nPairs));
+    size_t total = 0;
+    for (int64_t i = 0; i < 2 * nPairs; i++) {
+        if (lens[i] > SNAPGPU_MAX_READ_LENGTH) return sg_fail("read longer than MAX_READ_LENGTH");
+        off[i] = total; total += lens[i];
+    }
+    if (nPairs > e->stagePairs) {
+        cudaFree(e->d_offsets); cudaFree(e->d_lens); cudaFree(e->d_results);
+        e->d_offsets = nullptr; e->d_lens = nullptr; e->d_results = nullptr; e->stagePairs = 0;
+        SG_CUDA(cudaMalloc((void **)&e->d_offsets, (size_t)nPairs * 16));
+        SG_CUDA(cudaMalloc((void **)&e->d_lens, (size_t)nPairs * 8));
+        SG_CUDA(cudaMalloc((void **)&e->d_results, (size_t)nPairs * sizeof(snapgpu_paired_result)));
+        e->stagePairs = nPairs;
+    }
+    if (total + 1 > e->stageBases) {
+        cudaFree(e->d_bases); cudaFree(e->d_quals);
+        e->d_bases = e->d_quals = nullptr; e->stageBases = 0;
+        SG_CUDA(cudaMalloc((void **)&e->d_bases, total + 1));
+        SG_CUDA(cudaMalloc((void **)&e->d_quals, total + 1));
+        e->stageBases = total + 1;
+    }
+    cudaStream_t st = a->stream;
+    bool contiguous = true;
+    for (int64_t i = 0; i < 2 * nPairs && contiguous; i++) contiguous = offsets[i] == offsets[0] + off[i];
+    if (contiguous) {
+        SG_CUDA(cudaMemcpyAsync(e->d_bases, bases + offsets[0], total, cudaMemcpyHostToDevice, st));
+        SG_CUDA(cudaMemcpyAsync(e->d_quals, quals + offsets[0], total, cudaMemcpyHostToDevice, st));
+    } else {
+        std::vector<char> b(total), q(total);
+        for (int64_t i = 0; i < 2 * nPairs; i++) {
+            memcpy(&b[off[i]], bases + offsets[i], lens[i]);
+            memcpy(&q[off[i]], quals + offsets[i], lens[i]);
+        }
+        SG_CUDA(cudaMemcpyAsync(e->d_bases, b.data(), total, cudaMemcpyHostToDevice, st));
+        SG_CUDA(cudaMemcpyAsync(e->d_quals, q.data(), total, cudaMemcpyHostToDevice, st));
+        SG_CUDA(cudaStreamSynchronize(st));
+    }
+    SG_CUDA(cudaMemcpyAsync(e->d_offsets, off.data(), (size_t)nPairs * 16, cudaMemcpyHostToDevice, st));
+    SG_CUDA(cudaMemcpyAsync(e->d_lens, lens, (size_t)nPairs * 8, cudaMemcpyHostToDevice, st));
+    SG_CUDA(cudaMemsetAsync(e->d_ctr, 0, sizeof(snapgpu_counters), st));
+    if (align_paired_ins(a, e, nPairs, e->d_bases, e->d_quals, e->d_offsets, e->d_lens, e->d_results, e->d_ctr, st)) {
+        const std::string keep = g_lastError;
+        cudaStreamSynchronize(st); cudaGetLastError();
+        g_lastError = keep;
+        return 1;
+    }
+    SG_CUDA(cudaMemcpyAsync(results, e->d_results, (size_t)nPairs * sizeof(snapgpu_paired_result), cudaMemcpyDeviceToHost, st));
+    SG_CUDA(cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(snapgpu_counters), cudaMemcpyDeviceToHost, st));
+    SG_CUDA(cudaStreamSynchronize(st));
+    if (snapgpu_aligner_check(a, nullptr)) return 1;
+    if (counters) {
+        int64_t *dst = (int64_t *)counters; const int64_t *src = (const int64_t *)e->h_ctr;
+        for (size_t k = 0; k < sizeof(snapgpu_counters) / 8; k++) dst[k] += src[k];
+    }
+    return 0;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -98,10 +98,11 @@ EXPORTS = [
     "snapgpu_lookup_seeds", "snapgpu_lookup_seeds_device", "snapgpu_measure_random_sector_rate", "snapgpu_aligner_create", "snapgpu_aligner_destroy", "snapgpu_align_single",
     "snapgpu_align_single_device", "snapgpu_align_single_secondary", "snapgpu_align_single_secondary_device", "snapgpu_paired_params_default", "snapgpu_paired_aligner_create", "snapgpu_align_paired",
     "snapgpu_align_paired_device", "snapgpu_aligner_check", "snapgpu_fastq_create", "snapgpu_fastq_destroy", "snapgpu_fastq_parse_device",
-    "snapgpu_fastq_parse", "snapgpu_sam_create", "snapgpu_sam_destroy", "snapgpu_sam_format_single", "snapgpu_sam_format_paired", "snapgpu_sam_format_single_device", "snapgpu_sam_format_paired_device", "snapgpu_sam_set_format", "snapgpu_sam_header", "snapgpu_bgzf_device", "snapgpu_bgzf_deflate_device", "snapgpu_bam_index_members_device", "snapgpu_sam_sort_device", "snapgpu_sam_last_record_count", "snapgpu_bam_markdup_device", "snapgpu_bam_index_device", "snapgpu_aligner_launch_count", "snapgpu_aligner_deferred_count", "snapgpu_test_lv", "snapgpu_test_ag", "snapgpu_test_lv_warp", "snapgpu_test_ag_warp",
+    "snapgpu_fastq_parse", "snapgpu_sam_create", "snapgpu_sam_destroy", "snapgpu_sam_format_single", "snapgpu_sam_format_paired", "snapgpu_sam_format_single_device", "snapgpu_sam_format_paired_device", "snapgpu_sam_set_format", "snapgpu_sam_header", "snapgpu_bgzf_device", "snapgpu_bgzf_deflate_device", "snapgpu_bam_index_members_device", "snapgpu_sam_sort_device", "snapgpu_sam_last_record_count", "snapgpu_bam_markdup_device", "snapgpu_bam_index_device", "snapgpu_aligner_launch_count", "snapgpu_aligner_deferred_count",
+    "snapgpu_spacing_create", "snapgpu_spacing_destroy", "snapgpu_spacing_get", "snapgpu_spacing_timing", "snapgpu_align_paired_ins", "snapgpu_align_paired_ins_device", "snapgpu_test_lv", "snapgpu_test_ag", "snapgpu_test_lv_warp", "snapgpu_test_ag_warp",
 ]
 
-ABI_VERSION = 8          # include/snapgpu.h SNAPGPU_ABI_VERSION this mirror was written against
+ABI_VERSION = 9          # include/snapgpu.h SNAPGPU_ABI_VERSION this mirror was written against
 _lib = None
 
 
@@ -151,6 +152,12 @@ def lib():
         L.snapgpu_paired_aligner_create.argtypes = [C.c_void_p, C.POINTER(Params), C.POINTER(PairedParams), C.c_int64, C.POINTER(C.c_void_p)]
         L.snapgpu_align_paired.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 6
         L.snapgpu_align_paired_device.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 7
+        L.snapgpu_spacing_create.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_void_p)]
+        L.snapgpu_spacing_destroy.argtypes = [C.c_void_p]
+        L.snapgpu_spacing_get.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_uint32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.snapgpu_spacing_timing.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_double)]
+        L.snapgpu_align_paired_ins.argtypes = [C.c_void_p, C.c_void_p, C.c_int64] + [C.c_void_p] * 6
+        L.snapgpu_align_paired_ins_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int64] + [C.c_void_p] * 7
         L.snapgpu_aligner_check.argtypes = [C.c_void_p, C.c_void_p]
         L.snapgpu_fastq_create.argtypes = [C.c_int, C.c_int64, C.c_int64, C.POINTER(C.c_void_p)]
         L.snapgpu_fastq_destroy.argtypes = [C.c_void_p]
@@ -463,6 +470,60 @@ class PairedAligner:
             self.handle = None
 
     def __del__(self):       # a handle dropped without close() must not keep its arenas (tens of GB of HBM) until the process ends
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class SpacingEstimator:
+    """Insert-size inference of `snap paired -ins` for one worker's stream of pairs (reference PairedAligner.cpp:889-925):
+    snapgpu_spacing_*.  `filter_flags` are AlignerOptions::filterFlags bits; `window` 0 is stock's 262144, other values are a
+    test seam."""
+
+    def __init__(self, aligner: "PairedAligner", filter_flags: int = 0, window: int = 0):
+        h = C.c_void_p()
+        _check(lib().snapgpu_spacing_create(aligner.handle, filter_flags, window, C.byref(h)))
+        self.handle = h
+        self.aligner = aligner
+
+    def get(self) -> dict:
+        mn, mx, s, u = C.c_int32(), C.c_uint32(), C.c_int64(), C.c_int64()
+        _check(lib().snapgpu_spacing_get(self.handle, C.byref(mn), C.byref(mx), C.byref(s), C.byref(u)))
+        return {"minSpacing": mn.value, "maxSpacing": mx.value, "samples": s.value, "updates": u.value}
+
+    def timing(self) -> dict:
+        n, t = C.c_int64(), C.c_double()
+        _check(lib().snapgpu_spacing_timing(self.handle, C.byref(n), C.byref(t)))
+        return {"subLaunches": n.value, "statSeconds": t.value}
+
+    def align(self, batch, out=None):
+        """Host buffers in, host results out: snapgpu_align_paired_ins, in calls of at most the aligner's max_batch_pairs."""
+        n_pairs = batch.n // 2
+        res = np.zeros(n_pairs, dtype=PAIRED_RESULT_DTYPE) if out is None else out[:n_pairs]
+        ctr = np.zeros(N_COUNTERS, dtype=np.int64)
+        done = 0
+        while done < n_pairs:
+            m = min(self.aligner.max_batch_pairs, n_pairs - done)
+            sub_off = batch.offsets[2 * done:2 * (done + m)]
+            sub_len = batch.lens[2 * done:2 * (done + m)]
+            _check(lib().snapgpu_align_paired_ins(self.aligner.handle, self.handle, m, _p(batch.bases), _p(batch.quals), _p(sub_off),
+                                                  _p(sub_len), C.c_void_p(res.ctypes.data + done * PAIRED_RESULT_DTYPE.itemsize), _p(ctr)))
+            done += m
+        return res, counters_dict(ctr)
+
+    def align_device(self, n_pairs, d_bases, d_quals, d_offsets, d_lens, d_results, d_counters=0, stream=0):
+        """Device pointers (ints) in: snapgpu_align_paired_ins_device (synchronises `stream` between its sub-launches)."""
+        _check(lib().snapgpu_align_paired_ins_device(self.aligner.handle, self.handle, n_pairs, C.c_void_p(d_bases), C.c_void_p(d_quals),
+                                                      C.c_void_p(d_offsets), C.c_void_p(d_lens), C.c_void_p(d_results), C.c_void_p(d_counters),
+                                                      C.c_void_p(stream)))
+
+    def close(self):
+        if self.handle:
+            lib().snapgpu_spacing_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
         try:
             self.close()
         except Exception:
